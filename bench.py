@@ -2,13 +2,15 @@
 """bench.py -- view-tuples/sec of the hot path on synthetic 5-view x 1024-keypoint tuples.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config cfg3|cfg2|cfg4|cfg5] [--tuples B]
+                    [--dump-outputs DIR]
 
 A *step* is one pass of the hot path over one batch of B synthetic units per GPU.  Default = BASELINE.json
 configs[2] (cfg3: ScanNet-shape 5-tuple, 1024 kpts, 28-layer matcher, confidence head, 10 x {w8pt + two-view BA},
 spanning tree, rotation averaging + LUD, global LM BA); --config cfg2 / cfg4 are the two-view workloads
 (configs[1] / [3]: pairs/sec at 1024 / 2048 kpts, w8pt_ba).  One JSON line on rank 0; see DESIGN.md §measurement
-for every field.  `--impl reference` times the CPU port of the reference path (oracle/) on the host cores --
-/root/reference does not exist on the GPU box.
+for every field.  `--impl reference` times the CPU port of the reference path (oracle/) on the host cores.
+`--dump-outputs DIR` writes what the last timed step returned (matcher outputs and poses) as DIR/<name>.npy, so that two
+builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -92,7 +94,23 @@ def make_inputs(cfg, seed, batch, kpts=None):
                                    height=cfg['height'], f=cfg['f'])
 
 
-TF32_PEAK_TFLOPS = 148 * 4096 * 1.965e9 / 1e12      # tcgen05 kind::tf32 issue floor x SMs x max SM clock
+TF32_FLOP_PER_CLK_SM = 2048      # dense tf32 wgmma rate of an H100 SM (f16: twice that)
+DUMP_MAX_ELEMS = 1 << 17          # per array in --dump-outputs: larger outputs are written as a fixed, seeded sample
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> tensor / ndarray.  Floating arrays as float32 (float64 stays float64), integer and boolean arrays
+    as float64 (exact).  An array with more than DUMP_MAX_ELEMS elements is written as the values at DUMP_MAX_ELEMS flat
+    indices drawn once from a generator seeded by its shape, in ascending order (same positions in every run)."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in sorted(arrays.items()):
+        a = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+        a = a.astype(np.float64 if (a.dtype == np.float64 or not np.issubdtype(a.dtype, np.floating)) else np.float32)
+        if a.size > DUMP_MAX_ELEMS:
+            rng = np.random.default_rng(list(a.shape))
+            a = a.reshape(-1)[np.sort(rng.choice(a.size, DUMP_MAX_ELEMS, replace=False))]
+        np.save(os.path.join(out_dir, name + '.npy'), a)
 
 
 def emit(line):
@@ -102,25 +120,13 @@ def emit(line):
     sys.stdout.flush()
 
 
-def load_traffic(workload, batch):
-    """Per-launch DRAM traffic of the dominant kernels from the committed ncu capture (profiles/ncu_traffic.json),
-    valid for the workload / batch size it was captured at."""
-    try:
-        t = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'ncu_traffic.json')))
-        if t.get('tuples_per_step') == batch and t.get('workload', 'scannet_5tuple_1024kpts_28layers_mvba') == workload:
-            return t['attention']['avg_bytes_per_launch'], t['sinkhorn']['avg_bytes_per_launch']
-    except Exception:
-        pass
-    return None, None
-
-
 def load_peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         d = json.load(open(p))
         return {'hbm_gbs': d['hbm_gbs'], 'tflops': d.get('bf16_tflops_sustained', d['bf16_tflops']),
                 'source': 'measured (MEASURED_PEAKS.json, bf16 sustained / copy)'}
-    return {'hbm_gbs': 6650.0, 'tflops': 1400.0, 'source': 'fallback (B200_PROFILING.md)'}
+    return {'hbm_gbs': 3350.0, 'tflops': 989.0, 'source': 'H100 SXM data sheet (HBM3, dense BF16), not measured'}
 
 
 class ClockSampler(threading.Thread):
@@ -444,8 +450,7 @@ def run_train_arm(args, cfg, rank, world, local):
         att_ms, att_n = prof['attention']
         # algorithmic work: forward QK^T + PV (4 N M D per view and layer) + the five products of a memory-efficient
         # backward (S recomputed once, dP = dO V^T, dQ = dS K, dK = dS^T Q, dV = P^T dO: 10 N M D) = 14 N M D.  The two
-        # backward kernels EXECUTE eight (S three times, dP twice); the lines committed as profiles/bench_r02_cfg5_*.json
-        # were taken with 18 N M D in this place.
+        # backward kernels EXECUTE eight (S three times, dP twice).
         att_flops = attention_flops(cfg) * B * 2 * (14.0 / 4.0)
         att_tflops = att_flops / (att_ms * 1e-3) / 1e12 if att_ms > 0 else 0.0
         line = {'metric': cfg['metric'], 'value': args.steps / (ms_dev * 1e-3), 'unit': cfg['unit'], 'n_gpus': world,
@@ -460,10 +465,9 @@ def run_train_arm(args, cfg, rank, world, local):
                 'e2e': {'value': args.steps / (ms_e2e * 1e-3), 'unit': cfg['unit'], 'h2d_bytes_per_step': h2d_bytes, 'd2h_bytes_per_step': 4,
                         'ms_per_step': ms_e2e / args.steps},
                 'gpu_launches': int(launches), 'clocks': sampler.summary(),
-                'roofline': {'kernel': 'attention forward (tcgen05 fp16x3) + backward (mma.sync TF32 x 3 split passes, flash-style recomputation)',
+                'roofline': {'kernel': 'attention forward (wgmma fp16x3) + backward (mma.sync TF32 x 3 split passes, flash-style recomputation)',
                              'bound': 'tensor', 'achieved': att_tflops, 'peak': peaks['tflops'], 'unit': 'TFLOP/s',
-                             'frac': att_tflops / peaks['tflops'], 'traffic': None, 'launches_timed': att_n, 'peak_source': peaks['source'],
-                             'note': 'the backward runs on the legacy mma.sync path with register fragments; its tcgen05 port is the next step'},
+                             'frac': att_tflops / peaks['tflops'], 'traffic': None, 'launches_timed': att_n, 'peak_source': peaks['source']},
                 'step_split_ms': {'forward+loss': round(float(split[0]), 3), 'backward': round(float(split[1]), 3),
                                   'allreduce+optimizer': round(float(split[2]), 3)},
                 'stage_ms_per_step': {k: round(v[0] / 2, 4) for k, v in prof.items() if v[1] > 0},
@@ -504,7 +508,10 @@ def main():
     ap.add_argument('--gemm-split', type=int, default=-1, choices=[-1, 0, 1],
                     help='operand planes of the mode-3 layer GEMMs (persistent kernel): 0 = tf32 hi/lo, 1 = fp16 hi/lo')
     ap.add_argument('--math-mode', type=int, default=3, choices=[0, 1, 3],
-                    help='3 = tcgen05 3xTF32 (fp32-faithful, default), 1 = tcgen05 single-pass TF32, 0 = fp32 CUDA cores')
+                    help='3 = fp32-faithful split operands on the tensor cores (default), 1 = single-pass TF32, 0 = fp32 CUDA cores')
+    ap.add_argument('--dump-outputs', default='', metavar='DIR',
+                    help='cfg2 / cfg3 / cfg4: write what the last timed step computed as DIR/<name>.npy (float32 / float64, '
+                         'seeded samples of large arrays)')
     args = ap.parse_args()
     cfg = CONFIGS[args.config]
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
@@ -574,7 +581,7 @@ def main():
 
     def step_device():
         res, pose = pipe(data_dev)
-        last['res'] = res
+        last['res'], last['pose'] = res, pose
         if world > 1:   # the per-rank loss is accumulated on the device; ONE all-reduce closes the timed region
             loss.add_(step_loss(pose))
         return pose
@@ -621,7 +628,7 @@ def main():
             loss.add_(step_loss(pose))
         return pose
 
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
 
     def timed(fn, steps):
         evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
@@ -661,6 +668,9 @@ def main():
     n0 = lib.mvm_launch_count()
     ms_dev, wall_dev = timed(step_device, args.steps)
     launches = lib.mvm_launch_count() - n0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict({'res_' + k: v for k, v in last['res'].items() if isinstance(v, torch.Tensor)},
+                                             **{'pose_' + k: v for k, v in last['pose'].items() if isinstance(v, torch.Tensor)}))
     staged.clear()                 # the first timed step stages its own inputs inside the timed region
     ms_e2e, wall_e2e = timed(step_e2e, args.steps)
     e2e_steps = [round(x, 2) for x in last['per_step_ms']]
@@ -694,7 +704,7 @@ def main():
         total_units = B * args.steps * world
         value = sharding.whole_job_throughput(B, args.steps, world, ms_dev)
         e2e = total_units / (ms_e2e * 1e-3)
-        traffic_att, traffic_sink = load_traffic(cfg['workload'], B)
+        traffic_att = traffic_sink = None     # DRAM traffic per launch: not measured
         att_ms, att_n = prof['attention']
         att_flops = attention_flops(cfg) * B * prof_steps                  # over the profiled steps
         att_tflops = att_flops / (att_ms * 1e-3) / 1e12 if att_ms > 0 else 0.0
@@ -705,7 +715,9 @@ def main():
         # over it per iteration; peak = SMs x 128 B/clk x SM clock (shared-memory datapath)
         onchip_gbs = 100 * 2 * N_KPTS * N_KPTS * 4 * n_prob / (sk_ms * 1e-3) / 1e9 if sk_ms > 0 else 0.0
         sm_mhz = clocks.get('sm_mhz') or 1965.0
-        smem_peak_gbs = 148 * 128 * sm_mhz * 1e6 / 1e9
+        n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
+        smem_peak_gbs = n_sm * 128 * sm_mhz * 1e6 / 1e9
+        tf32_peak_tflops = n_sm * TF32_FLOP_PER_CLK_SM * (clocks.get('sm_max_mhz') or sm_mhz) * 1e6 / 1e12
         stage_ms = {k: round(v[0] / prof_steps, 4) for k, v in prof.items() if v[1] > 0}
         # pose AUC of the engine on the bench units (informational; engine-vs-oracle parity below and in tests/)
         if is_tuple:
@@ -718,18 +730,18 @@ def main():
                 errs.append(max(compute_pose_error_np(gt, Tp[i, :3, :3], Tp[i, :3, 3])) if ok[i] else np.inf)
         auc = pose_auc(np.array(errs), [5, 10, 20])
         last_res = last['res']
-        # issue-rate ceiling of the arithmetic the attention kernel really runs: kind::tf32 = 4096 FLOP/clk/SM, kind::f16
+        # issue-rate ceiling of the arithmetic the attention kernel really runs: tf32 wgmma = 2048 FLOP/clk/SM, f16
         # twice that; the fp32-faithful modes spend three MMAs per product
         if args.math_mode == 3:
-            ceiling = (2.0 if opt.attention_split == 1 else 1.0) * TF32_PEAK_TFLOPS / 3.0
+            ceiling = (2.0 if opt.attention_split == 1 else 1.0) * tf32_peak_tflops / 3.0
             ceiling_name = 'fp16x3' if opt.attention_split == 1 else 'tf32x3'
         else:
-            ceiling, ceiling_name = TF32_PEAK_TFLOPS, 'tf32'
+            ceiling, ceiling_name = tf32_peak_tflops, 'tf32'
 
         line = {
             'metric': cfg['metric'], 'value': value, 'unit': cfg['unit'], 'n_gpus': world, 'steps': args.steps,
             'warmup': args.warmup, 'ms_per_step': ms_dev / args.steps, 'higher_is_better': True, 'scaling': 'weak',
-            'vs_baseline': None, 'dtype': {3: 'f32 via split operands on tcgen05 (fp16x3 / tf32x3, fp32-faithful) / f64 pose kernels', 1: 'tf32 on tcgen05 / f64 pose kernels',
+            'vs_baseline': None, 'dtype': {3: 'f32 via split operands on the tensor cores (fp16x3 / tf32x3, fp32-faithful) / f64 pose kernels', 1: 'tf32 on the tensor cores / f64 pose kernels',
                       0: 'f32 CUDA cores / f64 pose kernels'}[args.math_mode], 'data': 'synthetic',
             'config': workload_config(cfg), 'units_per_step': B * world,
             'run': {'units_per_step_per_gpu': B, 'l2': 'flushed between timed steps (256 MB write)',
@@ -746,14 +758,14 @@ def main():
                          'achieved': att_tflops, 'peak': peaks['tflops'], 'unit': 'TFLOP/s',
                          'frac': att_tflops / peaks['tflops'], 'traffic': traffic_att, 'launches_timed': att_n,
                          'peak_source': peaks['source'],
-                         # the path computes in tf32 (half the bf16 rate: M128.N.K8 every N/2 cycles = 4096 FLOP/clk/SM)
-                         # and needs three passes to stay fp32-faithful: the reachable algorithmic ceiling
+                         # the path computes in tf32 / fp16 split operands and needs three passes to stay
+                         # fp32-faithful: the reachable algorithmic ceiling
                          'ceiling': ceiling, 'ceiling_arithmetic': ceiling_name, 'frac_of_ceiling': att_tflops / ceiling},
             'roofline_sinkhorn': {'kernel': 'sinkhorn (%d pairs x %d problems per launch)' % (P, B),
                                   'bound': 'on-chip (K~ resident in registers + shared memory; not HBM)',
                                   'achieved': onchip_gbs, 'peak': smem_peak_gbs, 'unit': 'GB/s',
                                   'frac': onchip_gbs / smem_peak_gbs, 'launches_timed': sk_n,
-                                  'peak_source': '148 SMs x 128 B/clk x sampled SM clock (shared-memory datapath)',
+                                  'peak_source': '%d SMs x 128 B/clk x sampled SM clock (shared-memory datapath)' % n_sm,
                                   # SURVEY.md 8(d)'s per-unit figure (the reference's HBM passes) over the same time
                                   'hbm_equivalent': {'achieved': sk_gbs, 'peak': peaks['hbm_gbs'], 'frac': sk_gbs / peaks['hbm_gbs'],
                                                      'unit': 'GB/s', 'traffic': traffic_sink}},
@@ -763,7 +775,7 @@ def main():
         }
         if tf32 is not None:
             line['tf32_single_pass'] = {'value': total_units / (tf32[0] * 1e-3), 'e2e': total_units / (tf32[1] * 1e-3),
-                                        'unit': cfg['unit'], 'note': 'math mode 1 (tcgen05 kind::tf32, one pass)'}
+                                        'unit': cfg['unit'], 'note': 'math mode 1 (tf32 wgmma, one pass)'}
         # quality of the synthetic assignment: fraction of returned matches that join the same landmark
         hits = tot = 0
         for b_ in range(T_VIEWS):
@@ -776,7 +788,7 @@ def main():
         line['match_precision'] = round(hits / max(tot, 1), 4)
         if world == 1 and not args.no_torch_gpu:
             # informational: the op-for-op torch port of the reference matcher run by stock PyTorch (cuBLAS / cuDNN
-            # eager) on the same GPU -- what a user of the reference gets by moving its model to the B200.  Matcher
+            # eager) on the same GPU -- what a user of the reference gets by moving its model to this GPU.  Matcher
             # only (the reference's pose stage is CPU code); our matcher-only rate from the stage timers beside it.
             try:
                 line['torch_gpu_port'] = torch_gpu_port(cfg, sd, data_np, dev, B, stage_ms)

@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) engine for the hot path of barbararoessle/e2e_multi_view_matching.
+"""H100-native (sm_90a) engine for the hot path of barbararoessle/e2e_multi_view_matching.
 
 Host-side mirror of the reference's Python interface for that path:
   models.multi_view_matcher.MultiViewMatcher   (models/models/multi_view_matcher.py:103)
@@ -13,8 +13,8 @@ __version__ = '0.1'
 
 
 def set_math_mode(mode):
-    """Math mode of the matcher's GEMMs/attention: 0 = fp32 CUDA cores, 3 = tcgen05 3xTF32
-    (fp32-faithful), 1 = tcgen05 single-pass TF32."""
+    """Math mode of the matcher's GEMMs/attention: 0 = fp32 CUDA cores, 3 = 3xTF32 on the tensor cores
+    (fp32-faithful), 1 = single-pass TF32."""
     from . import _lib
     _lib.check(_lib.lib().mvm_set_math_mode(int(mode)), 'mvm_set_math_mode')
 

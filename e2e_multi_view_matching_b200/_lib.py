@@ -2,7 +2,7 @@
 
 There is no CPU fallback: if the shared library is missing or a call returns a non-zero
 status this module raises.  Build it with ``python -m e2e_multi_view_matching_b200.build``
-(nvcc, sm_100a) -- __graft_entry__.build() does that.
+(nvcc, sm_90a) -- __graft_entry__.build() does that.
 """
 import ctypes as C
 import os

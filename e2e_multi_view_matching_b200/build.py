@@ -1,4 +1,4 @@
-"""Build libmvm_b200.so (all CUDA kernels + the C ABI) for sm_100a with nvcc, in-tree.
+"""Build libmvm_b200.so (all CUDA kernels + the C ABI) for sm_90a with nvcc, in-tree.
 
 Usage: python -m e2e_multi_view_matching_b200.build [--force]
 The shared library is written next to this file so that it travels to the GPU box with the
@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libmvm_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
          '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 
@@ -72,7 +72,7 @@ def build(force=False, verbose=False):
             print('==', s)
             print(log)
     objs = [o for o, _ in results]
-    cmd = [NVCC, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB] + objs + ['-lcuda']
+    cmd = [NVCC, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB] + objs + ['-lcuda']
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n%s\n%s' % (r.stdout, r.stderr))

@@ -1,840 +1,16 @@
-// Flash-style multi-head attention on the 5th-gen tensor cores, fp32-faithful with HALF-PRECISION operand planes
-// ("fp16x3"): every product is A_hi.B_hi + A_hi.B_lo + A_lo.B_hi with hi = fp16(x), lo = fp16(x - hi), fp32
-// accumulation in tensor memory.  hi + lo carries 22 mantissa bits -- the same as the tf32 hi/lo pair of
-// attention_tc.cu (measured: identical error on the same operands, DESIGN.md) -- but tcgen05.mma kind::f16 moves
-// K = 16 per instruction where kind::tf32 moves K = 8, so the three passes cost 1.5 tf32 passes: 768 tensor
-// cycles per 64-key tile instead of 1536.  (fp16 subnormals keep lo exact to 2^-24 absolute; operands of this
-// path -- projected descriptors, softmax numerators <= 2^8 -- are far inside the fp16 range.)
-// Reference semantics: attention() superglue.py:87-91, MultiHeadedAttention :94-109, cross source = concatenation
-// of the other views (multi_view_matcher.py:76-78,92-95).  prob[B,4,N,M] is never materialised.
-//
-// Same structure as attention_tc.cu: one CTA = 128 queries of one (view, head), key tiles of 64;
-//   warp 0      TMA producer: K_hi | K_lo and V_hi | V_lo [64 keys x 64 d] fp16 tiles (8 KB each, one 128-byte swizzle
-//               row per key), 3-deep rings; the planes are written by the QKV GEMM epilogue.  V is read KEY-major, i.e.
-//               as an MN-major B operand of P.V (instruction-descriptor bit 16): no transposed copy of V exists
-//   warp 1      tcgen05.mma issuer S = Q K^T   (M128 N64 K16 kind::f16, A = Q_hi / Q_lo from tensor memory)
-//   warp 2      tcgen05.mma issuer O_g += P V  (A = P_hi / P_lo from tensor memory)
-//   warps 3-6 / 7-10   softmax groups 0 / 1 (even / odd key tiles): thread r owns query row r; S row -> registers,
-//               exp2, P split into packed half2 hi / lo planes written OVER S in tensor memory (32 + 32 columns),
-//               per-group output accumulator resident in TMEM with lazy rescaling, merged once at the end.
-// S and P do NOT share tensor-memory columns (the half-precision P planes are small): the S buffer of a group is free
-// again as soon as its softmax threads have read the row into registers (barrier s_free), so Q K^T of the group's next
-// tile is issued under the exponentials of the current one instead of after its P V product.
-// TMEM columns: S0 [0,64)  S1 [64,128)  O0 [128,192)  O1 [192,256)  Q_hi [256,288)  Q_lo [288,320)
-//               P0 hi|lo [320,384)  P1 hi|lo [384,448).
-#include "common.cuh"
-#include "kernels.cuh"
-#include "tc_common.cuh"
-#include <cuda_fp16.h>
+// fp32-faithful multi-head attention with HALF-PRECISION operand planes ("fp16x3"): every product is
+// A_hi.B_hi + A_hi.B_lo + A_lo.B_hi with hi = fp16(x), lo = fp16(x - hi), fp32 accumulation.  hi + lo carries 22
+// mantissa bits -- the same as the tf32 hi/lo pair of attention_tc.cu -- but an f16 wgmma moves K = 16 per instruction
+// where tf32 moves K = 8, so the three passes cost 1.5 tf32 passes.  (fp16 subnormals keep lo exact to 2^-24 absolute;
+// operands of this path -- projected descriptors, softmax numerators <= 2^15 -- are far inside the fp16 range.)
+// The kernel is attn_wg::attention_wg_kernel<16> (attention_wg.cuh): K_hi | K_lo and V_hi | V_lo [64 keys x 64 d] fp16
+// tiles by TMA from the planes the QKV GEMM epilogue writes; V is read key-major as an MN-major B operand.
+#include "attention_wg.cuh"
 
-extern long long* g_attn_dbg;   // attention_tc.cu (mvm_debug_set_attention_timing)
-// 0 = two softmax groups, one CTA per SM; 1 = one softmax group, two CTAs per SM (attention_h3s_kernel)
+// Kernel variant of the fp16-plane attention (mvm_debug_set_attention_h3_variant).  This build has one kernel; the
+// setting is kept so that callers of the A/B hook keep working, and both values run it.
 int g_attn_h3_variant = 1;
 extern "C" void mvm_debug_set_attention_h3_variant(int v) { g_attn_h3_variant = v ? 1 : 0; }
-
-namespace {
-
-constexpr int BQ = 128, BKV = 64, HD = 64;
-constexpr int K_BYTES = BKV * HD * 2;         //  8 KB  [64 keys x 64 d] fp16, 128-byte rows
-constexpr int V_BYTES = BKV * HD * 2;         //  8 KB  [64 keys x 64 d] fp16 (MN-major B operand of P.V)
-
-struct HCfg {
-  // K and V^T ring depth.  The clock trace showed the Q K^T issuer waiting ~770 clk per tile for K with a 3-deep ring:
-  // a TMA load lands ~2 us after it is requested under this load, and the tile period settled at latency / depth.
-  static constexpr int ST = 6;
-  static constexpr int OFF_K = 0;                       // per stage: hi | lo
-  static constexpr int OFF_V = OFF_K + ST * K_BYTES * 2;
-  static constexpr int OFF_BAR = OFF_V + ST * V_BYTES * 2;
-  static constexpr int OFF_ML = OFF_BAR + 512;          // (m, l) of both softmax groups: float [2][2][128]
-  static constexpr int SMEM_BYTES = OFF_ML + 2048 + 1024;
-  static constexpr int NTHREADS = 352;
-  static constexpr int TMEM_COLS = 512;                 // 448 used (allocation sizes are powers of two)
-  static constexpr int MAX_TILES = 256;                 // key tiles per query view: 7 segments x 2048 keys / 64 = 224
-};
-
-struct AttnH3Args {
-  const float* qkv;    // [V, n_pad, 768]
-  float* out;          // [V, n_pad, 256]
-  int n_pad;
-  AttnSegs segs;
-  int is_cross;
-  long long* dbg;      // optional clock64 trace of CTA (0,0,0): [tile][16] (tools/attn_timing.py)
-};
-
-
-__device__ __forceinline__ float ex2_ftz(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-// x -> (hi, lo) half-precision planes of two consecutive elements, packed the way the tensor core reads a 16-bit A
-// operand from tensor memory (element k in the low half of 32-bit column k / 2)
-__device__ __forceinline__ void split_pack(float x0, float x1, uint32_t& hi, uint32_t& lo) {
-  const __half2 h = __floats2half2_rn(x0, x1);
-  const float2 hf = __half22float2(h);
-  const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {   // D = F32, A = B = F16, both K-major
-  return (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-// the same with the B operand MN-major (cute::UMMA::InstrDescriptor b_major_, bit 16): B tile stored [K rows][N
-// contiguous], here V [keys][64 d] with 128-byte swizzled rows -- 8 keys per 1024-byte swizzle atom (SBO = 1024), one
-// K = 16 step = 2 atoms = 2048 bytes
-__host__ __device__ constexpr uint32_t make_idesc_f16_bmn(int M, int N) { return make_idesc_f16(M, N) | (1u << 16); }
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 32 lanes x 16 columns store
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-
-// 32 lanes x 8 columns load / store (the rare accumulator rescale of the two-CTA kernel: few live registers)
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float* v) {
-  const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-
-__global__ void __launch_bounds__(HCfg::NTHREADS, 1)
-attention_h3_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                    const __grid_constant__ CUtensorMap tmKlo, const __grid_constant__ CUtensorMap tmVlo,
-                    const __grid_constant__ AttnH3Args g) {
-  using C_ = HCfg;
-  constexpr int ST = C_::ST;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_::OFF_BAR);
-  uint64_t* q_ready = bars + 0;             // Q rows stored to tensor memory (128 arrivals)
-  uint64_t* k_full = bars + 1;              // [ST]
-  uint64_t* k_empty = k_full + ST;          // [ST]
-  uint64_t* v_full = k_empty + ST;          // [ST]
-  uint64_t* v_empty = v_full + ST;          // [ST]
-  uint64_t* s_full = v_empty + ST;          // [2]  S(j) landed in TMEM
-  uint64_t* p_ready = s_full + 2;           // [2]  keys 0-31 of P(j) stored (128 arrivals)
-  uint64_t* o_full = p_ready + 2;           // [2]  P.V(j) landed in the TMEM accumulator of the tile's group
-  uint64_t* p_ready_b = o_full + 2;         // [2]  keys 32-63 of P(j) stored
-  uint64_t* s_free = p_ready_b + 2;         // [2]  S(j) read into registers by the softmax group (128 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(s_free + 2);
-  static_assert((1 + 4 * ST + 10 + 1) * 8 <= 512, "barrier area");
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bool trace_cta = g.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-  const bool trace = trace_cta && lane == 0;
-  // slots 6,7,13-15 are written from inside elect_one() regions (whichever lane was elected)
-  auto mark = [&](int tile, int slot) { if ((slot == 6 || slot == 7 || slot >= 13 ? trace_cta : trace) && tile < 64) g.dbg[tile * 16 + slot] = clock64(); };
-  // CTA-level trace (second half of the debug buffer): [cta][8] = smid, start, setup done, Q stored, first S read,
-  // last tile done, merged + stored
-  const int cta_lin = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
-  // producer timeline (third region of the debug buffer): [tile][4] = K wait done, K requested, V wait done, V requested
-  auto pmark = [&](int tile, int slot) { if (trace_cta && tile < 64) g.dbg[64 * 16 + 2048 * 8 + tile * 4 + slot] = clock64(); };
-  auto cmark = [&](int slot) {
-    if (g.dbg != nullptr && cta_lin < 2048) g.dbg[64 * 16 + cta_lin * 8 + slot] = clock64();
-  };
-  if (threadIdx.x == 0 && g.dbg != nullptr && cta_lin < 2048) {
-    uint32_t smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    g.dbg[64 * 16 + cta_lin * 8 + 0] = smid;
-    cmark(1);
-  }
-  const int q0 = blockIdx.x * BQ;
-  const int h = blockIdx.y;
-  const int v = blockIdx.z;
-  const int T = g.segs.n_views;
-  const int t = v % T, b = v / T;
-  if (q0 >= g.segs.counts[t]) return;
-
-  // softmax group 0 (warps 3-6) owns the Q rows: issue their global loads first, so the latency runs under the
-  // barrier / TMEM set-up below (measured: 4.7k of a CTA's 130k cycles went to a serial Q load)
-  float qr[HD];
-  if (warp >= 3 && warp < 7) {
-    const int qrow = (warp & 3) * 32 + lane;
-    const float4* qg = reinterpret_cast<const float4*>(g.qkv + ((long long)v * g.n_pad + q0 + qrow) * 768 + h * HD);
-    const bool in_range = (long long)v * g.n_pad + q0 + qrow < (long long)gridDim.z * g.n_pad;
-#pragma unroll
-    for (int i = 0; i < HD / 4; ++i) {
-      const float4 x = in_range ? __ldg(qg + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-      qr[4 * i] = x.x; qr[4 * i + 1] = x.y; qr[4 * i + 2] = x.z; qr[4 * i + 3] = x.w;
-    }
-  }
-
-  // flattened key-tile list of this query view: segments (views) in ascending order, 64 keys per tile
-  int nt = 0;
-  for (int s = 0; s < T; ++s) {
-    if (g.is_cross ? (s == t) : (s != t)) continue;
-    nt += (g.segs.counts[s] + BKV - 1) / BKV;
-  }
-  auto tile_info = [&](int j, int& seg, int& k0, int& cnt) {
-    int acc = 0;
-    for (int s = 0; s < T; ++s) {
-      if (g.is_cross ? (s == t) : (s != t)) continue;
-      const int n = (g.segs.counts[s] + BKV - 1) / BKV;
-      if (j < acc + n) { seg = s; k0 = (j - acc) * BKV; cnt = g.segs.counts[s]; return; }
-      acc += n;
-    }
-    seg = 0; k0 = 0; cnt = 0;
-  };
-
-  // Tile table, filled once by the whole CTA: the producer warp shares its scheduler with two softmax warps, and
-  // recomputing (segment, offset) with loops and divisions for every K and V tile made its ~400 instructions per
-  // tile the bottleneck of the fp16 kernel (clock trace r02: the producer issued a tile's loads 1.5 k cycles apart,
-  // the MMA issuer waited 800 cycles per tile for K).  One shared-memory load per tile instead.
-  __shared__ int s_krow[C_::MAX_TILES];       // row of the tile's first key in the K and V planes
-  for (int j = threadIdx.x; j < nt; j += C_::NTHREADS) {
-    int seg, k0, cnt;
-    tile_info(j, seg, k0, cnt);
-    s_krow[j] = (b * T + seg) * g.n_pad + k0;
-  }
-
-  auto sK = [&](int s) { return smem + C_::OFF_K + s * K_BYTES * 2; };
-  auto sV = [&](int s) { return smem + C_::OFF_V + s * V_BYTES * 2; };
-
-  if (threadIdx.x == 0) {
-    tc::mbar_init(q_ready, 128);
-    for (int i = 0; i < ST; ++i) {
-      tc::mbar_init(k_full + i, 1); tc::mbar_init(k_empty + i, 1);
-      tc::mbar_init(v_full + i, 1); tc::mbar_init(v_empty + i, 1);
-    }
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(s_full + i, 1); tc::mbar_init(p_ready + i, 128); tc::mbar_init(p_ready_b + i, 128); }
-    tc::mbar_init(o_full, 1); tc::mbar_init(o_full + 1, 1);
-    tc::mbar_init(s_free, 128); tc::mbar_init(s_free + 1, 128);
-    tc::fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) {
-    tc::prefetch_tmap(&tmK); tc::prefetch_tmap(&tmV);
-    tc::prefetch_tmap(&tmKlo); tc::prefetch_tmap(&tmVlo);
-  }
-  if (warp == 1) tc::tmem_alloc<C_::TMEM_COLS>(tmem_slot);
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  if (threadIdx.x == 0) cmark(2);
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S0 = tmem_base, tmem_O = tmem_base + 128, tmem_O1 = tmem_base + 192;
-  const uint32_t tmem_Q = tmem_base + 256, tmem_Qlo = tmem_base + 288, tmem_P0 = tmem_base + 320;
-
-  if (warp == 0) {
-    // =========================== TMA producer ===========================
-    auto load_K = [&](int j) {
-      const int s = j % ST;
-      tc::mbar_wait(k_empty + s, ((j / ST) & 1) ^ 1);
-      if (lane == 0) pmark(j, 0);
-      if (tc::elect_one()) {
-        tc::mbar_arrive_expect_tx(k_full + s, K_BYTES * 2);
-        const int krow = s_krow[j];
-        tc::tma_load_2d(sK(s), &tmK, k_full + s, h * HD, krow);
-        tc::tma_load_2d(sK(s) + K_BYTES, &tmKlo, k_full + s, h * HD, krow);
-      }
-      __syncwarp();
-      if (lane == 0) pmark(j, 1);
-    };
-    auto load_V = [&](int j) {
-      const int s = j % ST;
-      tc::mbar_wait(v_empty + s, ((j / ST) & 1) ^ 1);
-      if (lane == 0) pmark(j, 2);
-      if (tc::elect_one()) {
-        tc::mbar_arrive_expect_tx(v_full + s, V_BYTES * 2);
-        const int krow = s_krow[j];
-        tc::tma_load_2d(sV(s), &tmV, v_full + s, h * HD, krow);
-        tc::tma_load_2d(sV(s) + V_BYTES, &tmVlo, v_full + s, h * HD, krow);
-      }
-      __syncwarp();
-      if (lane == 0) pmark(j, 3);
-    };
-    load_K(0);
-    for (int j = 0; j < nt; ++j) {
-      load_V(j);
-      if (j + 1 < nt) load_K(j + 1);
-    }
-  } else if (warp == 1) {
-    // =========================== MMA issuer 1: S = Q K^T ===========================
-    // Two issuing warps, one per product.  A single issuer is serial -- barrier waits (~100 clk each even when
-    // the barrier has long completed), tcgen05.commit (~30-120 clk) and N=64 MMAs that execute in 32 clk, with
-    // a queue only a few entries deep: measured 2200 clk per key tile for 1536 clk of tensor work
-    // (tools/attn_timing.py).  With two instruction streams each warp's stalls are covered by the other's
-    // queued MMAs.  The ordering a single in-order stream gave for free is now explicit: S(j) overwrites the
-    // buffer P(j-2) was read from, so it waits for P.V(j-2) to complete (o_full[j & 1]).
-    // Whole warp converged, one elected lane issues (see tc::elect_one).
-    constexpr uint32_t idesc = make_idesc_f16(BQ, BKV);        // M=128, N=64
-    tc::mbar_wait(q_ready, 0);
-    tc::tc_fence_after();
-    for (int j = 0; j < nt; ++j) {
-      const int s = j % ST, sb = j & 1;
-      mark(j, 8);
-      tc::mbar_wait(k_full + s, (j / ST) & 1);
-      mark(j, 9);                      // K landed; what follows until slot 6 is the S-buffer wait + the issue
-      // S(j-2) of this buffer has been read into registers by its softmax group.  S(j) cannot have been read yet
-      // (it is not written), so the barrier is at most one phase ahead of the phase awaited: the parity wait is sound.
-      if (j >= 2) tc::mbar_wait(s_free + sb, ((j - 2) >> 1) & 1);
-      tc::tc_fence_after();
-      const uint32_t k_hi = tc::smem_u32(sK(s)), k_lo = k_hi + K_BYTES;
-      const uint32_t d = tmem_S0 + sb * 64;
-      if (tc::elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < HD / 16; ++kk) {                  // K = 16 halves = 32 bytes = 8 TMEM columns per MMA
-          const uint64_t dk = tc::make_kmajor_sw128_desc(k_hi + kk * 32);
-          umma_f16_ts(d, tmem_Q + kk * 8, dk, idesc, kk != 0);                // A = Q from tensor memory
-          umma_f16_ts(d, tmem_Q + kk * 8, tc::make_kmajor_sw128_desc(k_lo + kk * 32), idesc, 1);
-          umma_f16_ts(d, tmem_Qlo + kk * 8, dk, idesc, 1);
-        }
-        mark(j, 6);
-        tc::umma_commit(s_full + sb);
-        tc::umma_commit(k_empty + s);
-        mark(j, 7);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 2) {
-    // =========================== MMA issuer 2: O_g += P V ===========================
-    constexpr uint32_t idesc = make_idesc_f16_bmn(BQ, HD);  // M=128, N=64 (d), B = V key-major         // M=128, N=64
-    for (int j = 0; j < nt; ++j) {
-      const int s = j % ST, sb = j & 1;
-      // P(j) arrives in two halves (keys 0-31, 32-63): the first 12 MMAs start while the softmax threads are
-      // still exponentiating the second half
-      tc::mbar_wait(p_ready + sb, (j >> 1) & 1);
-      tc::mbar_wait(v_full + s, (j / ST) & 1);
-      tc::tc_fence_after();
-      mark(j, 10);
-      const uint32_t v_hi = tc::smem_u32(sV(s)), v_lo = v_hi + V_BYTES;
-      const uint32_t p_hi = tmem_P0 + sb * 64, p_lo = p_hi + 32;          // P planes of the group: hi [0,32) lo [32,64)
-      const uint32_t o_acc = sb ? tmem_O1 : tmem_O;
-      auto issue_PV = [&](int kk0) {                                       // two K = 16 steps = 32 keys
-#pragma unroll
-        for (int kk = kk0; kk < kk0 + 2; ++kk) {
-          const uint64_t dv = tc::make_kmajor_sw128_desc(v_hi + kk * 2048);   // 16 keys x 128 B
-          umma_f16_ts(o_acc, p_hi + kk * 8, dv, idesc, ((j >> 1) | kk) != 0);  // A = P from tensor memory; O_g accumulates over the group's tiles
-          umma_f16_ts(o_acc, p_hi + kk * 8, tc::make_kmajor_sw128_desc(v_lo + kk * 2048), idesc, 1);
-          umma_f16_ts(o_acc, p_lo + kk * 8, dv, idesc, 1);
-        }
-      };
-      if (tc::elect_one()) issue_PV(0);
-      __syncwarp();
-      mark(j, 11);
-      tc::mbar_wait(p_ready_b + sb, (j >> 1) & 1);
-      tc::tc_fence_after();
-      mark(j, 12);
-      if (tc::elect_one()) {
-        issue_PV(2);
-        mark(j, 13);
-        tc::umma_commit(o_full + (j & 1));
-        mark(j, 14);
-        tc::umma_commit(v_empty + s);
-        mark(j, 15);
-      }
-      __syncwarp();
-    }
-  } else {
-    // =========================== softmax groups ===========================
-    const int grp = warp >= 7 ? 1 : 0;
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(q * 32) << 16;
-    // group 0: Q row -> tensor memory (A operand of S = Q K^T); rows past the view are read but never written back
-    if (grp == 0) {
-      uint32_t qh[32], ql[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) split_pack(qr[2 * i], qr[2 * i + 1], qh[i], ql[i]);
-      tmem_st16(tmem_Q + lane_addr, qh);
-      tmem_st16(tmem_Q + lane_addr + 16, qh + 16);
-      tmem_st16(tmem_Qlo + lane_addr, ql);
-      tmem_st16(tmem_Qlo + lane_addr + 16, ql + 16);
-      tc::tmem_st_wait();
-      tc::tc_fence_before();
-      tc::mbar_arrive(q_ready);
-      if (warp == 3 && lane == 0) cmark(3);
-    }
-    // Online softmax over this group's key tiles (j = grp, grp + 2, ...) with the output accumulator RESIDENT IN
-    // TENSOR MEMORY.  The reference m_ref of a row is only raised (and O_g, l rescaled) when the row maximum
-    // outgrows it by more than 2^8: softmax is invariant to the reference, P stays <= 2^8, and the common tile
-    // costs no TMEM read of O at all.  Log2 units throughout (scores * log2(e) / sqrt(d)).
-    const uint32_t tm_S = tmem_S0 + grp * 64, tm_P = tmem_P0 + grp * 64, tm_O = grp ? tmem_O1 : tmem_O;
-    uint64_t* my_o_full = o_full + grp;
-    float m_ref = -INFINITY, l_run = 0.f;
-    const float scale_l2e = 0.125f * 1.4426950408889634f;
-    int j = 0, mine = 0;           // global tile index, tiles this group has processed
-    for (int sg = 0; sg < T; ++sg) {
-      if (g.is_cross ? (sg == t) : (sg != t)) continue;
-      const int cnt = g.segs.counts[sg];
-      for (int k0 = 0; k0 < cnt; k0 += BKV, ++j) {
-        if ((j & 1) != grp) continue;
-        const int nvalid = cnt - k0;      // keys of this tile that exist
-        if (q == 3) mark(j, 0);
-        tc::mbar_wait(s_full + grp, mine & 1);
-        tc::tc_fence_after();
-        if (q == 3) mark(j, 1);
-        if (warp == 3 && lane == 0 && j == 0) cmark(4);
-        float s[BKV];
-        tc::tmem_ld32(tm_S + lane_addr, s);
-        tc::tmem_ld32(tm_S + lane_addr + 32, s + 32);
-        tc::tmem_ld_wait();
-        tc::tc_fence_before();
-        tc::mbar_arrive(s_free + grp);          // the S buffer may be overwritten by Q K^T of tile j + 2
-        if (q == 3) mark(j, 2);
-        if (nvalid < BKV) {
-#pragma unroll
-          for (int i = 0; i < BKV; ++i) s[i] = (i < nvalid) ? s[i] : -INFINITY;
-        }
-        float mx4[4] = {s[0], s[1], s[2], s[3]};          // four independent chains instead of one of 63
-#pragma unroll
-        for (int i = 4; i < BKV; ++i) mx4[i & 3] = fmaxf(mx4[i & 3], s[i]);
-        const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3])) * scale_l2e;
-        const bool grow = mx > m_ref + 8.f;
-        if (__any_sync(0xffffffffu, grow)) {
-          float f = 1.f;
-          if (grow) { f = ex2_ftz(m_ref - mx); m_ref = mx; l_run *= f; }
-          if (mine > 0) {
-            // the group's previous product P.V(j-2) has landed: S(j), issued after it, has been read (the tensor
-            // pipe is in order); the wait only makes that visible to this thread
-            tc::mbar_wait(my_o_full, (mine - 1) & 1);
-            tc::tc_fence_after();
-            float o[32];
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              tc::tmem_ld32(tm_O + lane_addr + c * 32, o);
-              tc::tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) o[i] *= f;
-              tc::tmem_st32(tm_O + lane_addr + c * 32, o);
-            }
-            tc::tmem_st_wait();
-          }
-        }
-        if (q == 3) mark(j, 3);
-        if (mine > 0 && !__any_sync(0xffffffffu, grow)) {
-          // P(j) overwrites the planes P.V(j-2) read: that product must have completed (it has, long ago, in the
-          // steady state -- it was issued one softmax period back)
-          tc::mbar_wait(my_o_full, (mine - 1) & 1);
-          tc::tc_fence_after();
-        }
-        const float nm = -m_ref;
-        float rs4[4] = {0.f, 0.f, 0.f, 0.f};
-        // P(j) overwrites S(j) in tensor memory (row r = lane r, keys along columns): A operand of P.V,
-        // handed over in two halves
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {                        // keys [32 c, 32 c + 32): 16 packed columns per plane
-          uint32_t ph[16], pl[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float p0 = ex2_ftz(fmaf(s[c * 32 + 2 * i], scale_l2e, nm));
-            const float p1 = ex2_ftz(fmaf(s[c * 32 + 2 * i + 1], scale_l2e, nm));
-            rs4[i & 1] += p0;
-            rs4[2 + (i & 1)] += p1;
-            split_pack(p0, p1, ph[i], pl[i]);
-          }
-          tmem_st16(tm_P + lane_addr + c * 16, ph);            // P_hi columns [0,32)
-          tmem_st16(tm_P + lane_addr + 32 + c * 16, pl);       // P_lo columns [32,64)
-          tc::tmem_st_wait();
-          tc::tc_fence_before();
-          tc::mbar_arrive((c == 0 ? p_ready : p_ready_b) + grp);
-          if (q == 3) mark(j, 4 + c);
-        }
-        l_run += (rs4[0] + rs4[1]) + (rs4[2] + rs4[3]);
-        ++mine;
-      }
-    }
-    // ---- merge the two partial softmaxes:  out = (O_0 w_0 + O_1 w_1) / (l_0 w_0 + l_1 w_1),  w_g = 2^(m_g - m)
-    if (mine > 0) {
-      tc::mbar_wait(my_o_full, (mine - 1) & 1);     // the group's last product (hence all of them) has landed
-      tc::tc_fence_after();
-    }
-    if (warp == 3 && lane == 0) cmark(5);
-    float* ml = reinterpret_cast<float*>(smem + C_::OFF_ML);
-    ml[(grp * 2 + 0) * 128 + row] = m_ref;
-    ml[(grp * 2 + 1) * 128 + row] = l_run;
-    tc::tc_fence_before();
-    asm volatile("bar.sync 2, 256;" ::: "memory");
-    tc::tc_fence_after();
-    const bool has1 = j > 1;                        // group 1 saw at least one tile (uniform over the CTA)
-    const float m0 = ml[0 * 128 + row], l0 = ml[1 * 128 + row];
-    const float m1 = has1 ? ml[2 * 128 + row] : -INFINITY, l1 = has1 ? ml[3 * 128 + row] : 0.f;
-    const float mm = fmaxf(m0, m1);
-    const float w0 = ex2_ftz(m0 - mm), w1 = has1 ? ex2_ftz(m1 - mm) : 0.f;
-    const float inv = 1.f / (l0 * w0 + l1 * w1);
-    // group g writes d in [32 g, 32 g + 32) of the row
-    float o0[32], o1[32];
-    tc::tmem_ld32(tmem_O + lane_addr + grp * 32, o0);
-    if (has1) tc::tmem_ld32(tmem_O1 + lane_addr + grp * 32, o1);
-    tc::tmem_ld_wait();
-    if (q0 + row < g.n_pad) {
-      const float a0 = w0 * inv, a1 = w1 * inv;
-      float4* o4 = reinterpret_cast<float4*>(g.out + ((long long)v * g.n_pad + q0 + row) * 256 + h * HD + grp * 32);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float4 r;
-        r.x = o0[4 * i] * a0; r.y = o0[4 * i + 1] * a0; r.z = o0[4 * i + 2] * a0; r.w = o0[4 * i + 3] * a0;
-        if (has1) {
-          r.x = fmaf(o1[4 * i], a1, r.x); r.y = fmaf(o1[4 * i + 1], a1, r.y);
-          r.z = fmaf(o1[4 * i + 2], a1, r.z); r.w = fmaf(o1[4 * i + 3], a1, r.w);
-        }
-        o4[i] = r;
-      }
-    }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) cmark(6);
-  if (warp == 1) tc::tmem_dealloc<C_::TMEM_COLS>(tmem_base);
-  if (threadIdx.x == 32) cmark(7);
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------
-// Two CTAs per SM, one softmax group each ("h3s").  The two-group kernel above keeps the tensor pipe busy inside the
-// key-tile loop, but every CTA pays ~14 k cycles outside it (barrier / TMEM set-up, Q load, pipeline fill, merge of
-// the two partial softmaxes, output store, CTA launch gap; clock trace profiles/r02_attn_timing_h3.txt) with the SM
-// idle: 18 % of a cross-attention CTA, 47 % of a self-attention CTA (16 key tiles).  Here a CTA is HALF of that
-// machine -- one softmax warpgroup, a 3-deep K/V ring (96 KB), 256 tensor-memory columns -- so two CTAs are resident
-// per SM and the set-up / drain of one runs under the key-tile loop of the other.  All key tiles of the query block
-// go through the one group, so there is no merge: out = O / l.
-// TMEM columns: S [0,64)  O [64,128)  Q_hi [128,160)  Q_lo [160,192)  P hi|lo [192,256).
-struct SCfg {
-  static constexpr int ST = 3;
-  static constexpr int OFF_K = 0;
-  static constexpr int OFF_V = OFF_K + ST * K_BYTES * 2;
-  static constexpr int OFF_BAR = OFF_V + ST * V_BYTES * 2;
-  static constexpr int OFF_TAB = OFF_BAR + 256;         // tile table: int [MAX_TILES]
-  static constexpr int MAX_TILES = HCfg::MAX_TILES;
-  static constexpr int SMEM_BYTES = OFF_TAB + MAX_TILES * 4 + 1024;
-  static constexpr int NTHREADS = 224;                  // producer, two MMA issuers, four softmax warps
-  static constexpr int TMEM_COLS = 256;
-  static constexpr int OUT_LD = HD + 4;                 // output staging row (floats): conflict-free float4 rows
-};
-static_assert(2 * (SCfg::SMEM_BYTES + 1024) <= 227 * 1024, "two CTAs per SM");
-static_assert(BQ * SCfg::OUT_LD * 4 <= SCfg::ST * K_BYTES * 2, "output staging fits in the K ring");
-
-__global__ void __launch_bounds__(SCfg::NTHREADS, 2)
-attention_h3s_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                     const __grid_constant__ CUtensorMap tmKlo, const __grid_constant__ CUtensorMap tmVlo,
-                    const __grid_constant__ AttnH3Args g) {
-  using C_ = SCfg;
-  constexpr int ST = C_::ST;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_::OFF_BAR);
-  uint64_t* q_ready = bars + 0;             // Q rows stored to tensor memory (128 arrivals)
-  uint64_t* k_full = bars + 1;              // [ST]
-  uint64_t* k_empty = k_full + ST;          // [ST]
-  uint64_t* v_full = k_empty + ST;          // [ST]
-  uint64_t* v_empty = v_full + ST;          // [ST]
-  uint64_t* s_full = v_empty + ST;          // S(j) landed in TMEM
-  uint64_t* s_free = s_full + 1;            // S(j) read into registers (128 arrivals)
-  uint64_t* p_ready = s_free + 1;           // keys 0-31 of P(j) stored (128 arrivals)
-  uint64_t* p_ready_b = p_ready + 1;        // keys 32-63 of P(j) stored
-  uint64_t* o_full = p_ready_b + 1;         // P.V(j) landed in the accumulator
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
-  static_assert((1 + 4 * ST + 5 + 1) * 8 <= 256, "barrier area");
-  int* s_krow = reinterpret_cast<int*>(smem + C_::OFF_TAB);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int cta_lin = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
-  auto cmark = [&](int slot) {
-    if (g.dbg != nullptr && cta_lin < 2048) g.dbg[64 * 16 + cta_lin * 8 + slot] = clock64();
-  };
-  if (threadIdx.x == 0 && g.dbg != nullptr && cta_lin < 2048) {
-    uint32_t smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    g.dbg[64 * 16 + cta_lin * 8 + 0] = smid;
-    cmark(1);
-  }
-  const int q0 = blockIdx.x * BQ;
-  const int h = blockIdx.y;
-  const int v = blockIdx.z;
-  const int T = g.segs.n_views;
-  const int t = v % T, b = v / T;
-  if (q0 >= g.segs.counts[t]) return;
-
-  // the softmax threads own the Q rows: global loads first, their latency runs under the set-up
-  float qr[HD];
-  if (warp >= 3) {
-    const int qrow = (warp & 3) * 32 + lane;
-    const float4* qg = reinterpret_cast<const float4*>(g.qkv + ((long long)v * g.n_pad + q0 + qrow) * 768 + h * HD);
-    const bool in_range = (long long)v * g.n_pad + q0 + qrow < (long long)gridDim.z * g.n_pad;
-#pragma unroll
-    for (int i = 0; i < HD / 4; ++i) {
-      const float4 x = in_range ? __ldg(qg + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-      qr[4 * i] = x.x; qr[4 * i + 1] = x.y; qr[4 * i + 2] = x.z; qr[4 * i + 3] = x.w;
-    }
-  }
-
-  // tile table (see attention_h3_kernel): key segments (views) in ascending order, 64 keys per tile
-  int nt = 0;
-  for (int s = 0; s < T; ++s) {
-    if (g.is_cross ? (s == t) : (s != t)) continue;
-    nt += (g.segs.counts[s] + BKV - 1) / BKV;
-  }
-  for (int j = threadIdx.x; j < nt; j += C_::NTHREADS) {
-    int acc = 0, seg = 0, k0 = 0;
-    for (int s = 0; s < T; ++s) {
-      if (g.is_cross ? (s == t) : (s != t)) continue;
-      const int n = (g.segs.counts[s] + BKV - 1) / BKV;
-      if (j < acc + n) { seg = s; k0 = (j - acc) * BKV; break; }
-      acc += n;
-    }
-    s_krow[j] = (b * T + seg) * g.n_pad + k0;
-  }
-
-  auto sK = [&](int s) { return smem + C_::OFF_K + s * K_BYTES * 2; };
-  auto sV = [&](int s) { return smem + C_::OFF_V + s * V_BYTES * 2; };
-
-  if (threadIdx.x == 0) {
-    tc::mbar_init(q_ready, 128);
-    for (int i = 0; i < ST; ++i) {
-      tc::mbar_init(k_full + i, 1); tc::mbar_init(k_empty + i, 1);
-      tc::mbar_init(v_full + i, 1); tc::mbar_init(v_empty + i, 1);
-    }
-    tc::mbar_init(s_full, 1); tc::mbar_init(s_free, 128);
-    tc::mbar_init(p_ready, 128); tc::mbar_init(p_ready_b, 128);
-    tc::mbar_init(o_full, 1);
-    tc::fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) {
-    tc::prefetch_tmap(&tmK); tc::prefetch_tmap(&tmV);
-    tc::prefetch_tmap(&tmKlo); tc::prefetch_tmap(&tmVlo);
-  }
-  if (warp == 1) tc::tmem_alloc<C_::TMEM_COLS>(tmem_slot);
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  if (threadIdx.x == 0) cmark(2);
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base, tmem_O = tmem_base + 64;
-  const uint32_t tmem_Q = tmem_base + 128, tmem_Qlo = tmem_base + 160, tmem_P = tmem_base + 192;
-
-  if (warp == 0) {
-    // =========================== TMA producer ===========================
-    auto load_K = [&](int j) {
-      const int s = j % ST;
-      tc::mbar_wait(k_empty + s, ((j / ST) & 1) ^ 1);
-      if (tc::elect_one()) {
-        tc::mbar_arrive_expect_tx(k_full + s, K_BYTES * 2);
-        const int krow = s_krow[j];
-        tc::tma_load_2d(sK(s), &tmK, k_full + s, h * HD, krow);
-        tc::tma_load_2d(sK(s) + K_BYTES, &tmKlo, k_full + s, h * HD, krow);
-      }
-      __syncwarp();
-    };
-    auto load_V = [&](int j) {
-      const int s = j % ST;
-      tc::mbar_wait(v_empty + s, ((j / ST) & 1) ^ 1);
-      if (tc::elect_one()) {
-        tc::mbar_arrive_expect_tx(v_full + s, V_BYTES * 2);
-        const int krow = s_krow[j];
-        tc::tma_load_2d(sV(s), &tmV, v_full + s, h * HD, krow);
-        tc::tma_load_2d(sV(s) + V_BYTES, &tmVlo, v_full + s, h * HD, krow);
-      }
-      __syncwarp();
-    };
-    load_K(0);
-    for (int j = 0; j < nt; ++j) {
-      load_V(j);
-      if (j + 1 < nt) load_K(j + 1);
-    }
-  } else if (warp == 1) {
-    // =========================== MMA issuer 1: S = Q K^T ===========================
-    constexpr uint32_t idesc = make_idesc_f16(BQ, BKV);
-    tc::mbar_wait(q_ready, 0);
-    tc::tc_fence_after();
-    for (int j = 0; j < nt; ++j) {
-      const int s = j % ST;
-      tc::mbar_wait(k_full + s, (j / ST) & 1);
-      if (j >= 1) tc::mbar_wait(s_free, (j - 1) & 1);           // S(j-1) is in the softmax threads' registers
-      tc::tc_fence_after();
-      const uint32_t k_hi = tc::smem_u32(sK(s)), k_lo = k_hi + K_BYTES;
-      if (tc::elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < HD / 16; ++kk) {
-          const uint64_t dk = tc::make_kmajor_sw128_desc(k_hi + kk * 32);
-          umma_f16_ts(tmem_S, tmem_Q + kk * 8, dk, idesc, kk != 0);
-          umma_f16_ts(tmem_S, tmem_Q + kk * 8, tc::make_kmajor_sw128_desc(k_lo + kk * 32), idesc, 1);
-          umma_f16_ts(tmem_S, tmem_Qlo + kk * 8, dk, idesc, 1);
-        }
-        tc::umma_commit(s_full);
-        tc::umma_commit(k_empty + s);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 2) {
-    // =========================== MMA issuer 2: O += P V ===========================
-    constexpr uint32_t idesc = make_idesc_f16_bmn(BQ, HD);  // M=128, N=64 (d), B = V key-major
-    for (int j = 0; j < nt; ++j) {
-      const int s = j % ST;
-      tc::mbar_wait(p_ready, j & 1);
-      tc::mbar_wait(v_full + s, (j / ST) & 1);
-      tc::tc_fence_after();
-      const uint32_t v_hi = tc::smem_u32(sV(s)), v_lo = v_hi + V_BYTES;
-      const uint32_t p_hi = tmem_P, p_lo = tmem_P + 32;
-      auto issue_PV = [&](int kk0) {
-#pragma unroll
-        for (int kk = kk0; kk < kk0 + 2; ++kk) {
-          const uint64_t dv = tc::make_kmajor_sw128_desc(v_hi + kk * 2048);   // 16 keys x 128 B
-          umma_f16_ts(tmem_O, p_hi + kk * 8, dv, idesc, (j | kk) != 0);
-          umma_f16_ts(tmem_O, p_hi + kk * 8, tc::make_kmajor_sw128_desc(v_lo + kk * 2048), idesc, 1);
-          umma_f16_ts(tmem_O, p_lo + kk * 8, dv, idesc, 1);
-        }
-      };
-      if (tc::elect_one()) issue_PV(0);
-      __syncwarp();
-      tc::mbar_wait(p_ready_b, j & 1);
-      tc::tc_fence_after();
-      if (tc::elect_one()) {
-        issue_PV(2);
-        tc::umma_commit(o_full);
-        tc::umma_commit(v_empty + s);
-      }
-      __syncwarp();
-    }
-  } else {
-    // =========================== softmax (one warpgroup, every key tile) ===========================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(q * 32) << 16;
-    {
-      uint32_t qh[32], ql[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) split_pack(qr[2 * i], qr[2 * i + 1], qh[i], ql[i]);
-      tmem_st16(tmem_Q + lane_addr, qh);
-      tmem_st16(tmem_Q + lane_addr + 16, qh + 16);
-      tmem_st16(tmem_Qlo + lane_addr, ql);
-      tmem_st16(tmem_Qlo + lane_addr + 16, ql + 16);
-      tc::tmem_st_wait();
-      tc::tc_fence_before();
-      tc::mbar_arrive(q_ready);
-      if (warp == 3 && lane == 0) cmark(3);
-    }
-    float m_ref = -INFINITY, l_run = 0.f;
-    const float scale_l2e = 0.125f * 1.4426950408889634f;
-    int j = 0;
-    for (int sg = 0; sg < T; ++sg) {
-      if (g.is_cross ? (sg == t) : (sg != t)) continue;
-      const int cnt = g.segs.counts[sg];
-      for (int k0 = 0; k0 < cnt; k0 += BKV, ++j) {
-        const int nvalid = cnt - k0;
-        tc::mbar_wait(s_full, j & 1);
-        tc::tc_fence_after();
-        if (warp == 3 && lane == 0 && j == 0) cmark(4);
-        float s[BKV];
-        tc::tmem_ld32(tmem_S + lane_addr, s);
-        tc::tmem_ld32(tmem_S + lane_addr + 32, s + 32);
-        tc::tmem_ld_wait();
-        tc::tc_fence_before();
-        tc::mbar_arrive(s_free);                 // Q K^T of tile j + 1 may overwrite S
-        if (nvalid < BKV) {
-#pragma unroll
-          for (int i = 0; i < BKV; ++i) s[i] = (i < nvalid) ? s[i] : -INFINITY;
-        }
-        float mx4[4] = {s[0], s[1], s[2], s[3]};
-#pragma unroll
-        for (int i = 4; i < BKV; ++i) mx4[i & 3] = fmaxf(mx4[i & 3], s[i]);
-        const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3])) * scale_l2e;
-        const bool grow = mx > m_ref + 8.f;
-        bool o_waited = false;
-        if (__any_sync(0xffffffffu, grow)) {
-          float f = 1.f;
-          if (grow) { f = ex2_ftz(m_ref - mx); m_ref = mx; l_run *= f; }
-          if (j > 0) {
-            tc::mbar_wait(o_full, (j - 1) & 1);   // P.V(j-1) has landed: the accumulator may be rescaled
-            tc::tc_fence_after();
-            o_waited = true;
-            // eight columns at a time: the S row stays in registers (this path is rare -- first tiles of a row)
-#pragma unroll 1
-            for (int c = 0; c < HD; c += 8) {
-              float o[8];
-              tmem_ld8(tmem_O + lane_addr + c, o);
-              tc::tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 8; ++i) o[i] *= f;
-              tmem_st8(tmem_O + lane_addr + c, o);
-            }
-            tc::tmem_st_wait();
-          }
-        }
-        const float nm = -m_ref;
-        float rs4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t ph[16], pl[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float p0 = ex2_ftz(fmaf(s[c * 32 + 2 * i], scale_l2e, nm));
-            const float p1 = ex2_ftz(fmaf(s[c * 32 + 2 * i + 1], scale_l2e, nm));
-            rs4[i & 1] += p0;
-            rs4[2 + (i & 1)] += p1;
-            split_pack(p0, p1, ph[i], pl[i]);
-          }
-          if (c == 0 && j > 0 && !o_waited) {
-            // P(j) overwrites the planes P.V(j-1) reads: wait for that product as late as possible
-            tc::mbar_wait(o_full, (j - 1) & 1);
-            tc::tc_fence_after();
-          }
-          tmem_st16(tmem_P + lane_addr + c * 16, ph);
-          tmem_st16(tmem_P + lane_addr + 32 + c * 16, pl);
-          tc::tmem_st_wait();
-          tc::tc_fence_before();
-          tc::mbar_arrive(c == 0 ? p_ready : p_ready_b);
-        }
-        l_run += (rs4[0] + rs4[1]) + (rs4[2] + rs4[3]);
-      }
-    }
-    // ---- out = O / l, staged through the (now idle) K ring so that the global stores are full 256-byte rows
-    if (j > 0) {
-      tc::mbar_wait(o_full, (j - 1) & 1);
-      tc::tc_fence_after();
-    }
-    if (warp == 3 && lane == 0) cmark(5);
-    const float inv = 1.f / l_run;
-    float* stage = reinterpret_cast<float*>(smem + C_::OFF_K);
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      float o[32];
-      tc::tmem_ld32(tmem_O + lane_addr + c * 32, o);
-      tc::tmem_ld_wait();
-      float4* d4 = reinterpret_cast<float4*>(stage + row * C_::OUT_LD + c * 32);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) d4[i] = make_float4(o[4 * i] * inv, o[4 * i + 1] * inv, o[4 * i + 2] * inv, o[4 * i + 3] * inv);
-    }
-    asm volatile("bar.sync 2, 128;" ::: "memory");
-    // warp q writes rows [32 q, 32 q + 32): one instruction = two rows of 64 floats
-    const int sub = lane >> 4, c4 = lane & 15;
-#pragma unroll 4
-    for (int i = 0; i < 16; ++i) {
-      const int r = q * 32 + 2 * i + sub;
-      if (q0 + r < g.n_pad) {
-        const float4 x = *reinterpret_cast<const float4*>(stage + r * C_::OUT_LD + c4 * 4);
-        *reinterpret_cast<float4*>(g.out + ((long long)v * g.n_pad + q0 + r) * 256 + h * HD + c4 * 4) = x;
-      }
-    }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) cmark(6);
-  if (warp == 1) tc::tmem_dealloc<C_::TMEM_COLS>(tmem_base);
-  if (threadIdx.x == 32) cmark(7);
-}
-
-}  // namespace
 
 // K / V planes in half precision: kh, kl, vh, vl [rows, 256] (written by the QKV GEMM epilogue)
 int launch_attention_h3(const float* qkv, const __half* kh, const __half* kl, const __half* vh, const __half* vl,
@@ -842,32 +18,11 @@ int launch_attention_h3(const float* qkv, const __half* kh, const __half* kl, co
   MVM_REQUIRE(qkv && kh && kl && vh && vl && out);
   MVM_REQUIRE(n_pad % 64 == 0 && segs.n_views >= 1 && segs.n_views <= 8);
   MVM_REQUIRE(!is_cross || segs.n_views >= 2);
-  MVM_REQUIRE((segs.n_views - 1) * (n_pad / 64) <= HCfg::MAX_TILES || !is_cross);
-  MVM_REQUIRE(n_pad / 64 <= HCfg::MAX_TILES);
   MvmProfScope prof__(MVM_TAG_ATTN, stream);
-  using C_ = HCfg;
-  mvm_once_per_device(MVM_ONCE_ATTN_H3, [&] {
-    cudaFuncSetAttribute(attention_h3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES);
-  });
-  const int V = batch * segs.n_views;
-  const long long rows = (long long)V * n_pad;
-  const CUtensorMap* tK = mvm_get_tmap_2d_f16(kh, rows, 256, 256, BKV);
-  const CUtensorMap* tKlo = mvm_get_tmap_2d_f16(kl, rows, 256, 256, BKV);
-  const CUtensorMap* tV = mvm_get_tmap_2d_f16(vh, rows, 256, 256, BKV);
-  const CUtensorMap* tVlo = mvm_get_tmap_2d_f16(vl, rows, 256, 256, BKV);
-  if (!tK || !tV || !tKlo || !tVlo) return MVM_ERR_LAUNCH;
-  AttnH3Args g;
-  g.qkv = qkv; g.out = out; g.n_pad = n_pad; g.segs = segs; g.is_cross = is_cross; g.dbg = g_attn_dbg;
-  dim3 grid(mvm_div_up(n_pad, BQ), 4, V);
-  if (g_attn_h3_variant == 1) {
-    mvm_once_per_device(MVM_ONCE_ATTN_H3S, [&] {
-      cudaFuncSetAttribute(attention_h3s_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SCfg::SMEM_BYTES);
-    });
-    attention_h3s_kernel<<<grid, SCfg::NTHREADS, SCfg::SMEM_BYTES, stream>>>(*tK, *tV, *tKlo, *tVlo, g);
-    MVM_CHECK_LAUNCH();
-    return MVM_OK;
-  }
-  attention_h3_kernel<<<grid, C_::NTHREADS, C_::SMEM_BYTES, stream>>>(*tK, *tV, *tKlo, *tVlo, g);
-  MVM_CHECK_LAUNCH();
-  return MVM_OK;
+  const long long rows = (long long)batch * segs.n_views * n_pad;
+  const CUtensorMap* tK = mvm_get_tmap_2d_f16(kh, rows, 256, 256, attn_wg::BKV);
+  const CUtensorMap* tKlo = mvm_get_tmap_2d_f16(kl, rows, 256, 256, attn_wg::BKV);
+  const CUtensorMap* tV = mvm_get_tmap_2d_f16(vh, rows, 256, 256, attn_wg::BKV);
+  const CUtensorMap* tVlo = mvm_get_tmap_2d_f16(vl, rows, 256, 256, attn_wg::BKV);
+  return attn_wg::launch<16>(tK, tV, tKlo, tVlo, qkv, out, batch, n_pad, segs, is_cross, stream);
 }

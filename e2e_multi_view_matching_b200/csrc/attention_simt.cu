@@ -2,7 +2,7 @@
 // (the probability tensor prob[B,4,N,M] of superglue.py:89-91 is never materialised).
 // Reference semantics: attention() superglue.py:87-91, MultiHeadedAttention :94-109,
 // cross source = concatenation of the other views, multi_view_matcher.py:76-78,92-95.
-// This is the exact-fp32 cross-check path; the tcgen05 kernel lives in attention_tc.cu.
+// This is the exact-fp32 cross-check path; the tensor-core kernels live in attention_wg.cuh.
 #include "common.cuh"
 #include "kernels.cuh"
 

@@ -1,488 +1,8 @@
-// Flash-style multi-head attention on the 5th-gen tensor cores (tcgen05 + TMEM + TMA) with
-// multi-view key/value segments.  Reference semantics: attention() superglue.py:87-91,
-// MultiHeadedAttention :94-109, cross source = concatenation of the other views
-// (multi_view_matcher.py:76-78,92-95).  prob[B,4,N,M] is never materialised.
-//
-// One CTA = 128 queries of one (view, head); keys/values stream through in tiles of 64.
-//   warp 0      TMA producer   per tile K [64x64] (from QKV) and V^T [64 d x 64 keys], 3-deep rings
-//   warp 1      tcgen05.mma issuer for S = Q K^T  (M128 N64 K64, kind::tf32) into one of two TMEM S buffers
-//   warp 2      tcgen05.mma issuer for O_g += P V (M128 N64 K64) into the TMEM accumulator of the tile's
-//               softmax group; BOTH A operands (Q and P) live in tensor memory, so shared-memory bandwidth
-//               only carries the K / V^T tiles
-//   warps 3-6   softmax group 0 (even key tiles), warps 7-10 softmax group 1 (odd key tiles): thread r of a
-//               group owns query row r (TMEM lane r): tcgen05.ld S row, row max / sum in registers (no
-//               shuffles), exp2, P written back to TENSOR MEMORY (tcgen05.st) and consumed as the A operand
-//               of P.V straight from TMEM.  Each group has its own S/P buffer, its own output accumulator in
-//               TMEM (O_g += P(j) V(j) over its tiles) and its own softmax reference (m_g, l_g); the two
-//               partial softmaxes are merged once at the end (exact: softmax is invariant to the reference).
-//               Two groups so that a tile's S -> softmax -> P latency (wake-up, TMEM load, 64 exp2, split, TMEM
-//               store: ~1.2 k cycles) overlaps the other group's tile instead of idling the tensor pipe
-//   (NPASS == 3) every product is A.B + A.B_lo + A_lo.B (fp32-faithful "3xTF32"): the tf32 hi/lo planes of
-//               K and V^T are produced by the QKV GEMM epilogue and arrive by TMA; Q and P are split in
-//               registers by the softmax threads before they are stored to tensor memory
-// All operands are K-major: Q, K rows of the fused QKV projection [rows, 768]; V^T [view*256 + h*64 + d, key]
-// is written by the QKV GEMM epilogue (gemm_tc.cu).
-#include "common.cuh"
-#include "kernels.cuh"
-#include "tc_common.cuh"
+// Multi-head attention on the tensor cores with tf32 operands (single pass, or 3xTF32 with the hi / lo planes of K and
+// V^T written by the QKV GEMM epilogue); the kernel is attn_wg::attention_wg_kernel (attention_wg.cuh).
+#include "attention_wg.cuh"
 
-long long* g_attn_dbg = nullptr;   // optional clock64 trace buffer (mvm_debug_set_attention_timing); shared with attention_h3.cu
-
-namespace {
-
-constexpr int BQ = 128, BKV = 64, HD = 64;
-constexpr int SUB = 32;                       // fp32 elements per 128-byte swizzle row
-constexpr int KV_SUB_BYTES = BKV * SUB * 4;   //  8 KB  [64 rows x 128 B]
-constexpr int K_BYTES = 2 * KV_SUB_BYTES;     // d 0-31 | d 32-63      (rows = keys)
-constexpr int V_BYTES = 2 * KV_SUB_BYTES;     // keys 0-31 | keys 32-63 (rows = d)
-
-template <int NPASS>
-struct ACfg {
-  static constexpr int ST = 3;                          // K and V^T ring depth
-  static constexpr int PL = NPASS == 3 ? 2 : 1;         // planes (hi [, lo])
-  static constexpr int OFF_K = 0;
-  static constexpr int OFF_V = OFF_K + ST * K_BYTES * PL;
-  static constexpr int OFF_BAR = OFF_V + ST * V_BYTES * PL;
-  static constexpr int OFF_ML = OFF_BAR + 512;          // (m, l) of both softmax groups: float [2][2][128]
-  static constexpr int SMEM_BYTES = OFF_ML + 2048 + 1024;
-  static constexpr int NTHREADS = 352;
-  static constexpr int MIN_CTAS = 1;
-  // TMEM columns: S0/P0 [0,64) S1/P1 [64,128) O0 [128,192) Q_hi [192,256)
-  //               Q_lo [256,320) P0_lo [320,384) P1_lo [384,448) O1 [448,512)
-  static constexpr int TMEM_COLS = 512;
-};
-
-struct AttnTcArgs {
-  const float* qkv;    // [V, n_pad, 768]
-  float* out;          // [V, n_pad, 256]
-  int n_pad;
-  AttnSegs segs;
-  int is_cross;
-  long long* dbg;      // optional clock64 trace of CTA (0,0,0): [tile][16] (tools/attn_timing.py)
-};
-
-using tc::tf32_rn;
-
-__device__ __forceinline__ float ex2_ftz(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-// rn_tf32 of a finite value with two integer instructions (round to nearest, ties away -- what cvt.rna does,
-// which the compiler expands to four instructions with the Inf/NaN guard)
-__device__ __forceinline__ float tf32_hi(float x) {
-  return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
-}
-
-template <int NPASS>
-__global__ void __launch_bounds__(ACfg<NPASS>::NTHREADS, ACfg<NPASS>::MIN_CTAS)
-attention_tc_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                    const __grid_constant__ CUtensorMap tmKlo, const __grid_constant__ CUtensorMap tmVlo,
-                    const __grid_constant__ AttnTcArgs g) {
-  using C_ = ACfg<NPASS>;
-  constexpr int ST = C_::ST;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_::OFF_BAR);
-  uint64_t* q_ready = bars + 0;    // Q rows stored to tensor memory (128 arrivals)
-  uint64_t* k_full = bars + 1;     // [ST]
-  uint64_t* k_empty = bars + 4;    // [ST]
-  uint64_t* k_split = bars + 7;    // [ST]
-  uint64_t* v_full = bars + 10;    // [ST]
-  uint64_t* v_empty = bars + 13;   // [ST]
-  uint64_t* v_split = bars + 16;   // [ST]
-  uint64_t* s_full = bars + 19;    // [2]  S(j) landed in TMEM
-  uint64_t* p_ready = bars + 21;   // [2]  keys 0-31 of P(j) stored over S(j) (128 arrivals)
-  uint64_t* p_ready_b = bars + 25; // [2]  keys 32-63 of P(j) stored
-  uint64_t* o_full = bars + 23;    // [2]  P.V(j) landed in the TMEM accumulator (alternating, see the softmax warps)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 28);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bool trace_cta = g.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-  const bool trace = trace_cta && lane == 0;
-  // slots 6,7,13-15 are written from inside elect_one() regions (whichever lane was elected)
-  auto mark = [&](int tile, int slot) { if ((slot == 6 || slot == 7 || slot >= 13 ? trace_cta : trace) && tile < 64) g.dbg[tile * 16 + slot] = clock64(); };
-  // CTA-level trace (second half of the debug buffer): [cta][8] = smid, start, setup done, Q stored, first S read,
-  // last tile done, merged + stored
-  const int cta_lin = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
-  auto cmark = [&](int slot) {
-    if (g.dbg != nullptr && cta_lin < 2048) g.dbg[64 * 16 + cta_lin * 8 + slot] = clock64();
-  };
-  if (threadIdx.x == 0 && g.dbg != nullptr && cta_lin < 2048) {
-    uint32_t smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    g.dbg[64 * 16 + cta_lin * 8 + 0] = smid;
-    cmark(1);
-  }
-  const int q0 = blockIdx.x * BQ;
-  const int h = blockIdx.y;
-  const int v = blockIdx.z;
-  const int T = g.segs.n_views;
-  const int t = v % T, b = v / T;
-  if (q0 >= g.segs.counts[t]) return;
-
-  // softmax group 0 (warps 3-6) owns the Q rows: issue their global loads first, so the latency runs under the
-  // barrier / TMEM set-up below (measured: 4.7k of a CTA's 130k cycles went to a serial Q load)
-  float qr[HD];
-  if (warp >= 3 && warp < 7) {
-    const int qrow = (warp & 3) * 32 + lane;
-    const float4* qg = reinterpret_cast<const float4*>(g.qkv + ((long long)v * g.n_pad + q0 + qrow) * 768 + h * HD);
-    const bool in_range = (long long)v * g.n_pad + q0 + qrow < (long long)gridDim.z * g.n_pad;
-#pragma unroll
-    for (int i = 0; i < HD / 4; ++i) {
-      const float4 x = in_range ? __ldg(qg + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-      qr[4 * i] = x.x; qr[4 * i + 1] = x.y; qr[4 * i + 2] = x.z; qr[4 * i + 3] = x.w;
-    }
-  }
-
-  // flattened key-tile list of this query view: segments (views) in ascending order, 64 keys per tile
-  int nt = 0;
-  for (int s = 0; s < T; ++s) {
-    if (g.is_cross ? (s == t) : (s != t)) continue;
-    nt += (g.segs.counts[s] + BKV - 1) / BKV;
-  }
-  auto tile_info = [&](int j, int& seg, int& k0, int& cnt) {
-    int acc = 0;
-    for (int s = 0; s < T; ++s) {
-      if (g.is_cross ? (s == t) : (s != t)) continue;
-      const int n = (g.segs.counts[s] + BKV - 1) / BKV;
-      if (j < acc + n) { seg = s; k0 = (j - acc) * BKV; cnt = g.segs.counts[s]; return; }
-      acc += n;
-    }
-    seg = 0; k0 = 0; cnt = 0;
-  };
-
-  auto sK = [&](int s) { return smem + C_::OFF_K + s * K_BYTES * C_::PL; };
-  auto sV = [&](int s) { return smem + C_::OFF_V + s * V_BYTES * C_::PL; };
-
-  if (threadIdx.x == 0) {
-    tc::mbar_init(q_ready, 128);
-    for (int i = 0; i < ST; ++i) {
-      tc::mbar_init(k_full + i, 1); tc::mbar_init(k_empty + i, 1); tc::mbar_init(k_split + i, 128);
-      tc::mbar_init(v_full + i, 1); tc::mbar_init(v_empty + i, 1); tc::mbar_init(v_split + i, 128);
-    }
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(s_full + i, 1); tc::mbar_init(p_ready + i, 128); tc::mbar_init(p_ready_b + i, 128); }
-    tc::mbar_init(o_full, 1); tc::mbar_init(o_full + 1, 1);
-    tc::fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) {
-    tc::prefetch_tmap(&tmK); tc::prefetch_tmap(&tmV);
-    if (NPASS == 3) { tc::prefetch_tmap(&tmKlo); tc::prefetch_tmap(&tmVlo); }
-  }
-  if (warp == 1) tc::tmem_alloc<C_::TMEM_COLS>(tmem_slot);
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  if (threadIdx.x == 0) cmark(2);
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S0 = tmem_base, tmem_O = tmem_base + 128, tmem_Q = tmem_base + 192;
-  const uint32_t tmem_Qlo = tmem_base + 256, tmem_Plo0 = tmem_base + 320, tmem_O1 = tmem_base + 448;
-
-  if (warp == 0) {
-    // =========================== TMA producer ===========================
-    auto load_K = [&](int j) {
-      int seg, k0, cnt;
-      tile_info(j, seg, k0, cnt);
-      const int s = j % ST;
-      tc::mbar_wait(k_empty + s, ((j / ST) & 1) ^ 1);
-      if (tc::elect_one()) {
-        tc::mbar_arrive_expect_tx(k_full + s, K_BYTES * C_::PL);
-        const int krow = (b * T + seg) * g.n_pad + k0;
-        tc::tma_load_2d(sK(s), &tmK, k_full + s, 256 + h * HD, krow);
-        tc::tma_load_2d(sK(s) + KV_SUB_BYTES, &tmK, k_full + s, 256 + h * HD + SUB, krow);
-        if (NPASS == 3) {
-          tc::tma_load_2d(sK(s) + K_BYTES, &tmKlo, k_full + s, h * HD, krow);
-          tc::tma_load_2d(sK(s) + K_BYTES + KV_SUB_BYTES, &tmKlo, k_full + s, h * HD + SUB, krow);
-        }
-      }
-      __syncwarp();
-    };
-    auto load_V = [&](int j) {
-      int seg, k0, cnt;
-      tile_info(j, seg, k0, cnt);
-      const int s = j % ST;
-      tc::mbar_wait(v_empty + s, ((j / ST) & 1) ^ 1);
-      if (tc::elect_one()) {
-        tc::mbar_arrive_expect_tx(v_full + s, V_BYTES * C_::PL);
-        const int vrow = (b * T + seg) * 256 + h * HD;
-        tc::tma_load_2d(sV(s), &tmV, v_full + s, k0, vrow);
-        tc::tma_load_2d(sV(s) + KV_SUB_BYTES, &tmV, v_full + s, k0 + SUB, vrow);
-        if (NPASS == 3) {
-          tc::tma_load_2d(sV(s) + V_BYTES, &tmVlo, v_full + s, k0, vrow);
-          tc::tma_load_2d(sV(s) + V_BYTES + KV_SUB_BYTES, &tmVlo, v_full + s, k0 + SUB, vrow);
-        }
-      }
-      __syncwarp();
-    };
-    load_K(0);
-    for (int j = 0; j < nt; ++j) {
-      load_V(j);
-      if (j + 1 < nt) load_K(j + 1);
-    }
-  } else if (warp == 1) {
-    // =========================== MMA issuer 1: S = Q K^T ===========================
-    // Two issuing warps, one per product.  A single issuer is serial -- barrier waits (~100 clk each even when
-    // the barrier has long completed), tcgen05.commit (~30-120 clk) and N=64 MMAs that execute in 32 clk, with
-    // a queue only a few entries deep: measured 2200 clk per key tile for 1536 clk of tensor work
-    // (tools/attn_timing.py).  With two instruction streams each warp's stalls are covered by the other's
-    // queued MMAs.  The ordering a single in-order stream gave for free is now explicit: S(j) overwrites the
-    // buffer P(j-2) was read from, so it waits for P.V(j-2) to complete (o_full[j & 1]).
-    // Whole warp converged, one elected lane issues (see tc::elect_one).
-    constexpr uint32_t idesc = tc::make_idesc_tf32(BQ, BKV);   // M=128, N=64
-    tc::mbar_wait(q_ready, 0);
-    tc::tc_fence_after();
-    for (int j = 0; j < nt; ++j) {
-      const int s = j % ST, sb = j & 1;
-      mark(j, 8);
-      tc::mbar_wait(k_full + s, (j / ST) & 1);
-      // P.V(j-2) done reading P / P_lo of this buffer.  P.V(j) cannot have completed (it needs this S), so the
-      // barrier is at most one phase ahead of the phase awaited: the parity wait is sound.
-      if (j >= 2) tc::mbar_wait(o_full + sb, ((j - 2) >> 1) & 1);
-      tc::tc_fence_after();
-      mark(j, 9);
-      const uint32_t k_hi = tc::smem_u32(sK(s)), k_lo = k_hi + K_BYTES;
-      const uint32_t d = tmem_S0 + sb * 64;
-      if (tc::elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < HD / 8; ++kk) {
-          const uint32_t offk = (kk >> 2) * KV_SUB_BYTES + (kk & 3) * 32;
-          const uint64_t dk = tc::make_kmajor_sw128_desc(k_hi + offk);
-          tc::umma_tf32_ts(d, tmem_Q + kk * 8, dk, idesc, kk != 0);           // A = Q from tensor memory
-          if (NPASS == 3) {
-            tc::umma_tf32_ts(d, tmem_Q + kk * 8, tc::make_kmajor_sw128_desc(k_lo + offk), idesc, 1);
-            tc::umma_tf32_ts(d, tmem_Qlo + kk * 8, dk, idesc, 1);
-          }
-        }
-        mark(j, 6);
-        tc::umma_commit(s_full + sb);
-        tc::umma_commit(k_empty + s);
-        mark(j, 7);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 2) {
-    // =========================== MMA issuer 2: O_g += P V ===========================
-    constexpr uint32_t idesc = tc::make_idesc_tf32(BQ, HD);    // M=128, N=64
-    for (int j = 0; j < nt; ++j) {
-      const int s = j % ST, sb = j & 1;
-      // P(j) arrives in two halves (keys 0-31, 32-63): the first 12 MMAs start while the softmax threads are
-      // still exponentiating the second half
-      tc::mbar_wait(p_ready + sb, (j >> 1) & 1);
-      tc::mbar_wait(v_full + s, (j / ST) & 1);
-      tc::tc_fence_after();
-      mark(j, 10);
-      const uint32_t v_hi = tc::smem_u32(sV(s)), v_lo = v_hi + V_BYTES;
-      const uint32_t p_hi = tmem_S0 + sb * 64, p_lo = tmem_Plo0 + sb * 64;
-      const uint32_t o_acc = sb ? tmem_O1 : tmem_O;
-      auto issue_PV = [&](int kk0) {
-#pragma unroll
-        for (int kk = kk0; kk < kk0 + BKV / 16; ++kk) {
-          const uint32_t offv = (kk >> 2) * KV_SUB_BYTES + (kk & 3) * 32;
-          const uint64_t dv = tc::make_kmajor_sw128_desc(v_hi + offv);
-          tc::umma_tf32_ts(o_acc, p_hi + kk * 8, dv, idesc, ((j >> 1) | kk) != 0);  // A = P from tensor memory; O_g accumulates over the group's tiles
-          if (NPASS == 3) {
-            tc::umma_tf32_ts(o_acc, p_hi + kk * 8, tc::make_kmajor_sw128_desc(v_lo + offv), idesc, 1);
-            tc::umma_tf32_ts(o_acc, p_lo + kk * 8, dv, idesc, 1);
-          }
-        }
-      };
-      if (tc::elect_one()) issue_PV(0);
-      __syncwarp();
-      mark(j, 11);
-      tc::mbar_wait(p_ready_b + sb, (j >> 1) & 1);
-      tc::tc_fence_after();
-      mark(j, 12);
-      if (tc::elect_one()) {
-        issue_PV(BKV / 16);
-        mark(j, 13);
-        tc::umma_commit(o_full + (j & 1));
-        mark(j, 14);
-        tc::umma_commit(v_empty + s);
-        mark(j, 15);
-      }
-      __syncwarp();
-    }
-  } else {
-    // =========================== softmax groups ===========================
-    const int grp = warp >= 7 ? 1 : 0;
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(q * 32) << 16;
-    // group 0: Q row -> tensor memory (A operand of S = Q K^T); rows past the view are read but never written back
-    if (grp == 0) {
-      if (NPASS == 3) {
-        float lo[32];
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float hi = tf32_rn(qr[c * 32 + i]);
-            lo[i] = tf32_rn(qr[c * 32 + i] - hi);
-            qr[c * 32 + i] = hi;
-          }
-          tc::tmem_st32(tmem_Qlo + lane_addr + c * 32, lo);
-        }
-      }
-      tc::tmem_st32(tmem_Q + lane_addr, qr);
-      tc::tmem_st32(tmem_Q + lane_addr + 32, qr + 32);
-      tc::tmem_st_wait();
-      tc::tc_fence_before();
-      tc::mbar_arrive(q_ready);
-      if (warp == 3 && lane == 0) cmark(3);
-    }
-    // Online softmax over this group's key tiles (j = grp, grp + 2, ...) with the output accumulator RESIDENT IN
-    // TENSOR MEMORY.  The reference m_ref of a row is only raised (and O_g, l rescaled) when the row maximum
-    // outgrows it by more than 2^8: softmax is invariant to the reference, P stays <= 2^8, and the common tile
-    // costs no TMEM read of O at all.  Log2 units throughout (scores * log2(e) / sqrt(d)).
-    const uint32_t tm_S = tmem_S0 + grp * 64, tm_Plo = tmem_Plo0 + grp * 64, tm_O = grp ? tmem_O1 : tmem_O;
-    uint64_t* my_o_full = o_full + grp;
-    float m_ref = -INFINITY, l_run = 0.f;
-    const float scale_l2e = 0.125f * 1.4426950408889634f;
-    int j = 0, mine = 0;           // global tile index, tiles this group has processed
-    for (int sg = 0; sg < T; ++sg) {
-      if (g.is_cross ? (sg == t) : (sg != t)) continue;
-      const int cnt = g.segs.counts[sg];
-      for (int k0 = 0; k0 < cnt; k0 += BKV, ++j) {
-        if ((j & 1) != grp) continue;
-        const int nvalid = cnt - k0;      // keys of this tile that exist
-        if (q == 3) mark(j, 0);
-        tc::mbar_wait(s_full + grp, mine & 1);
-        tc::tc_fence_after();
-        if (q == 3) mark(j, 1);
-        if (warp == 3 && lane == 0 && j == 0) cmark(4);
-        float s[BKV];
-        tc::tmem_ld32(tm_S + lane_addr, s);
-        tc::tmem_ld32(tm_S + lane_addr + 32, s + 32);
-        tc::tmem_ld_wait();
-        if (q == 3) mark(j, 2);
-        if (nvalid < BKV) {
-#pragma unroll
-          for (int i = 0; i < BKV; ++i) s[i] = (i < nvalid) ? s[i] : -INFINITY;
-        }
-        float mx4[4] = {s[0], s[1], s[2], s[3]};          // four independent chains instead of one of 63
-#pragma unroll
-        for (int i = 4; i < BKV; ++i) mx4[i & 3] = fmaxf(mx4[i & 3], s[i]);
-        const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3])) * scale_l2e;
-        const bool grow = mx > m_ref + 8.f;
-        if (__any_sync(0xffffffffu, grow)) {
-          float f = 1.f;
-          if (grow) { f = ex2_ftz(m_ref - mx); m_ref = mx; l_run *= f; }
-          if (mine > 0) {
-            // the group's previous product P.V(j-2) has landed: S(j), issued after it, has been read (the tensor
-            // pipe is in order); the wait only makes that visible to this thread
-            tc::mbar_wait(my_o_full, (mine - 1) & 1);
-            tc::tc_fence_after();
-            float o[32];
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              tc::tmem_ld32(tm_O + lane_addr + c * 32, o);
-              tc::tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) o[i] *= f;
-              tc::tmem_st32(tm_O + lane_addr + c * 32, o);
-            }
-            tc::tmem_st_wait();
-          }
-        }
-        if (q == 3) mark(j, 3);
-        const float nm = -m_ref;
-        float rs4[4] = {0.f, 0.f, 0.f, 0.f};
-        // P(j) overwrites S(j) in tensor memory (row r = lane r, keys along columns): A operand of P.V,
-        // handed over in two halves
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          float lo[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float pv = ex2_ftz(fmaf(s[c * 32 + i], scale_l2e, nm));
-            rs4[i & 3] += pv;
-            if (NPASS == 3) {
-              const float hi = tf32_hi(pv);
-              lo[i] = pv - hi;          // the tensor core reads the top 19 bits: truncation of lo costs 2^-21 |p|
-              s[c * 32 + i] = hi;
-            } else {
-              s[c * 32 + i] = pv;
-            }
-          }
-          if (NPASS == 3) tc::tmem_st32(tm_Plo + lane_addr + c * 32, lo);
-          tc::tmem_st32(tm_S + lane_addr + c * 32, s + c * 32);
-          tc::tmem_st_wait();
-          tc::tc_fence_before();
-          tc::mbar_arrive((c == 0 ? p_ready : p_ready_b) + grp);
-          if (q == 3) mark(j, 4 + c);
-        }
-        l_run += (rs4[0] + rs4[1]) + (rs4[2] + rs4[3]);
-        ++mine;
-      }
-    }
-    // ---- merge the two partial softmaxes:  out = (O_0 w_0 + O_1 w_1) / (l_0 w_0 + l_1 w_1),  w_g = 2^(m_g - m)
-    if (mine > 0) {
-      tc::mbar_wait(my_o_full, (mine - 1) & 1);     // the group's last product (hence all of them) has landed
-      tc::tc_fence_after();
-    }
-    if (warp == 3 && lane == 0) cmark(5);
-    float* ml = reinterpret_cast<float*>(smem + C_::OFF_ML);
-    ml[(grp * 2 + 0) * 128 + row] = m_ref;
-    ml[(grp * 2 + 1) * 128 + row] = l_run;
-    tc::tc_fence_before();
-    asm volatile("bar.sync 2, 256;" ::: "memory");
-    tc::tc_fence_after();
-    const bool has1 = j > 1;                        // group 1 saw at least one tile (uniform over the CTA)
-    const float m0 = ml[0 * 128 + row], l0 = ml[1 * 128 + row];
-    const float m1 = has1 ? ml[2 * 128 + row] : -INFINITY, l1 = has1 ? ml[3 * 128 + row] : 0.f;
-    const float mm = fmaxf(m0, m1);
-    const float w0 = ex2_ftz(m0 - mm), w1 = has1 ? ex2_ftz(m1 - mm) : 0.f;
-    const float inv = 1.f / (l0 * w0 + l1 * w1);
-    // group g writes d in [32 g, 32 g + 32) of the row
-    float o0[32], o1[32];
-    tc::tmem_ld32(tmem_O + lane_addr + grp * 32, o0);
-    if (has1) tc::tmem_ld32(tmem_O1 + lane_addr + grp * 32, o1);
-    tc::tmem_ld_wait();
-    if (q0 + row < g.n_pad) {
-      const float a0 = w0 * inv, a1 = w1 * inv;
-      float4* o4 = reinterpret_cast<float4*>(g.out + ((long long)v * g.n_pad + q0 + row) * 256 + h * HD + grp * 32);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float4 r;
-        r.x = o0[4 * i] * a0; r.y = o0[4 * i + 1] * a0; r.z = o0[4 * i + 2] * a0; r.w = o0[4 * i + 3] * a0;
-        if (has1) {
-          r.x = fmaf(o1[4 * i], a1, r.x); r.y = fmaf(o1[4 * i + 1], a1, r.y);
-          r.z = fmaf(o1[4 * i + 2], a1, r.z); r.w = fmaf(o1[4 * i + 3], a1, r.w);
-        }
-        o4[i] = r;
-      }
-    }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) cmark(6);
-  if (warp == 1) tc::tmem_dealloc<C_::TMEM_COLS>(tmem_base);
-  if (threadIdx.x == 32) cmark(7);
-}
-
-template <int NPASS>
-int launch_attn(const float* qkv, const float* vt, const float* klo, const float* vtlo, float* out, int batch, int n_pad,
-                const AttnSegs& segs, int is_cross, cudaStream_t stream) {
-  using C_ = ACfg<NPASS>;
-  mvm_once_per_device(MVM_ONCE_ATTN_TC + 16 * (NPASS == 3), [&] {
-    cudaFuncSetAttribute(attention_tc_kernel<NPASS>, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES);
-  });
-  const int V = batch * segs.n_views;
-  const long long rows = (long long)V * n_pad;
-  const CUtensorMap* tK = mvm_get_tmap_2d(qkv, rows, 768, 768, BKV);
-  const CUtensorMap* tV = mvm_get_tmap_2d(vt, (long long)V * 256, n_pad, n_pad, BKV);
-  const CUtensorMap* tKlo = klo ? mvm_get_tmap_2d(klo, rows, 256, 256, BKV) : tK;
-  const CUtensorMap* tVlo = vtlo ? mvm_get_tmap_2d(vtlo, (long long)V * 256, n_pad, n_pad, BKV) : tV;
-  if (!tK || !tV || !tKlo || !tVlo) return MVM_ERR_LAUNCH;
-  AttnTcArgs g;
-  g.qkv = qkv; g.out = out; g.n_pad = n_pad; g.segs = segs; g.is_cross = is_cross; g.dbg = g_attn_dbg;
-  dim3 grid(mvm_div_up(n_pad, BQ), 4, V);
-  attention_tc_kernel<NPASS><<<grid, C_::NTHREADS, C_::SMEM_BYTES, stream>>>(*tK, *tV, *tKlo, *tVlo, g);
-  MVM_CHECK_LAUNCH();
-  return MVM_OK;
-}
-
-}  // namespace
+long long* g_attn_dbg = nullptr;   // clock64 trace buffer of mvm_debug_set_attention_timing (no kernel of this build writes it)
 
 extern "C" void mvm_debug_set_attention_timing(long long* buf) { g_attn_dbg = buf; }
 
@@ -492,9 +12,15 @@ int launch_attention_tc(const float* qkv, const float* vt, float* out, int batch
   MVM_REQUIRE(n_pad % 64 == 0 && segs.n_views >= 1 && segs.n_views <= 8);
   MVM_REQUIRE(!is_cross || segs.n_views >= 2);
   MvmProfScope prof__(MVM_TAG_ATTN, stream);
+  const int V = batch * segs.n_views;
+  const long long rows = (long long)V * n_pad;
+  const CUtensorMap* tK = mvm_get_tmap_2d(qkv, rows, 768, 768, attn_wg::BKV);
+  const CUtensorMap* tV = mvm_get_tmap_2d(vt, (long long)V * 256, n_pad, n_pad, attn_wg::HD);
   if (n_pass == 3) {
     MVM_REQUIRE(klo && vtlo);
-    return launch_attn<3>(qkv, vt, klo, vtlo, out, batch, n_pad, segs, is_cross, stream);
+    const CUtensorMap* tKlo = mvm_get_tmap_2d(klo, rows, 256, 256, attn_wg::BKV);
+    const CUtensorMap* tVlo = mvm_get_tmap_2d(vtlo, (long long)V * 256, n_pad, n_pad, attn_wg::HD);
+    return attn_wg::launch<3>(tK, tV, tKlo, tVlo, qkv, out, batch, n_pad, segs, is_cross, stream);
   }
-  return launch_attn<1>(qkv, vt, nullptr, nullptr, out, batch, n_pad, segs, is_cross, stream);
+  return attn_wg::launch<1>(tK, tV, tK, tV, qkv, out, batch, n_pad, segs, is_cross, stream);
 }

@@ -220,7 +220,8 @@ extern "C" int mvm_batchnorm_train(const float* x, float* y, int rows, int C, in
   cudaStream_t s = (cudaStream_t)stream;
   MvmProfScope prof__(MVM_TAG_MISC, s);
   const int threads = ((C + 31) / 32) * 32;
-  const int blocks = rows < 592 ? rows : 592;                 // 4 x 148
+  const int max_blocks = 4 * mvm_dev_info().n_sm;
+  const int blocks = rows < max_blocks ? rows : max_blocks;
   const int rpb = (rows + blocks - 1) / blocks;
   const long long count = (long long)(rows / n_pad / slot_mod) * n_valid;
   bn_shift_kernel<<<(C + 255) / 256, 256, 0, s>>>(x, C, (long long)slot_rem * n_pad * ld, ws);

@@ -68,7 +68,7 @@ struct DevBuf {
 
 void need_gpu() {
   int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n < 1) die("no CUDA device: this binary only runs the sm_100a solvers", 3);
+  if (cudaGetDeviceCount(&n) != cudaSuccess || n < 1) die("no CUDA device: this binary only runs the sm_90a solvers", 3);
 }
 
 // 12 fields per camera: rotation column-major then translation (ba_problem.cpp:97-113, ba_init.cpp:58-75)

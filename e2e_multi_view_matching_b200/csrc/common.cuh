@@ -1,4 +1,4 @@
-// Shared device/host helpers for the sm_100a kernels of the matcher + pose hot path.
+// Shared device/host helpers for the sm_90a kernels of the matcher + pose hot path.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -79,7 +79,7 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   return v;
 }
 
-// ---- GEMM descriptor shared by the SIMT and tcgen05 paths ------------------------------
+// ---- GEMM descriptor shared by the SIMT and tensor-core paths ------------------------------
 // C[M,N] = act(alpha * [A | A2][M,K] * W[N,K]^T + bias[N]) + R[M,N]
 // A covers k in [0,K1), A2 covers k in [K1,K) (concat-by-K-split; A2 == nullptr -> K1 == K).
 struct GemmDesc {
@@ -87,7 +87,7 @@ struct GemmDesc {
   const float* A2; int lda2; int K1;
   const float* W;  int ldw;
   const float* Whi; const float* Wlo;          // optional pre-split tf32 planes of W (3xTF32 mode)
-  const void* Whi16; const void* Wlo16;        // optional half-precision planes of wscale * W (fp16x3 mode, persistent kernel)
+  const void* Whi16; const void* Wlo16;        // optional half-precision planes of wscale * W (fp16x3 mode, persistent schedule)
   float wscale;
   const float* bias;
   const float* R;  int ldr;

@@ -1,6 +1,6 @@
 // fp32 CUDA-core GEMM with fused epilogue (bias, ReLU, residual, concat-by-K-split).
 // Exact-fp32 path used for (a) small/odd shapes (score matrix with ldc = n+1, keypoint
-// encoder) and (b) as the on-device cross-check of the tcgen05 path.
+// encoder) and (b) as the on-device cross-check of the tensor-core path.
 // Replaces the reference's nn.Conv1d(k=1)+BatchNorm1d(eval)+ReLU chains
 // (superglue.py:51-62,101-121; multi_view_matcher.py:8-53) on point-major activations.
 #include "common.cuh"

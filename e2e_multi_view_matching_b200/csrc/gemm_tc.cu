@@ -1,240 +1,390 @@
-// tcgen05 GEMM with fused epilogue for the 1x1 convolutions of the matcher
-// (superglue.py:51-62,101-121; multi_view_matcher.py:8-53):
-//   C[M,N] = act(alpha * [A | A2][M,K] . W[N,K]^T + bias[N]) + R[M,N]      (all fp32, K-major)
+// Tensor-core GEMM (sm_90a: TMA + mbarrier ring + wgmma) with fused epilogue for the 1x1 convolutions of the matcher
+// (superglue.py:51-62,101-121; multi_view_matcher.py:8-53) and for its score matrices (multi_view_matcher.py:278-280):
+//   C[M,N] = act(alpha * [A | A2][M,K] . W[N,K]^T + bias[N]) + R[M,N]      (fp32, both operands K-major)
 //
-// Warp roles (192 threads, one 128 x BN output tile per CTA):
-//   warp 0      TMA producer: cp.async.bulk.tensor 128B-swizzled [128 x 32] A and [BN x 32] W tiles
-//               into a STAGES-deep ring (mbarrier expect_tx / complete_tx)
-//   warp 1      TMEM allocator + single-thread tcgen05.mma issuer (kind::tf32, M = 128, N = BN,
-//               K = 8 per instruction, accumulator in TMEM), tcgen05.commit frees the ring slots
-//   warps 2-5   (NPASS == 3) operand splitters during the main loop: lo = x - tf32(x) of every
-//               landed tile into a second smem buffer, so that D += A.W + A.W_lo + A_lo.W
-//               reproduces fp32 products to ~2^-21 (the "3xTF32" scheme) with no extra HBM traffic;
-//               then the epilogue: tcgen05.ld 32x32b -> registers -> bias/ReLU/residual -> global
-// NPASS == 1 is the single-pass TF32 mode (what torch 1.10 did by default on Ampere+).
+// Operand arithmetic (template parameters NPASS, WM):
+//   NPASS 1             single-pass TF32 (what torch 1.10 did by default on Ampere+)
+//   NPASS 3, W_RAW      3xTF32: D += A_hi.W_hi + A_hi.W_lo + A_lo.W_hi, hi = rn_tf32(x), lo = rn_tf32(x - hi); the W tile
+//                       is split into its hi / lo planes in shared memory after it lands
+//   NPASS 3, W_TF32     3xTF32 with W given as its two tf32 planes (what packing.py stores next to the raw weights)
+//   NPASS 3, W_F16      fp16x3: W given as fp16 hi / lo planes of wscale * W (packing.py), A split into fp16 hi / lo;
+//                       the same 22-bit operands, K = 16 per instruction instead of 8
+// A is split on chip in every mode: it is the register operand of wgmma, so its hi / lo planes never touch shared memory.
+//
+// One CTA computes 128 x BN output tiles with 288 threads:
+//   warps 0-3, 4-7   two consumer warpgroups, tile rows [0,64) and [64,128): A fragments from the 128B-swizzled shared
+//                    tile -> hi / lo in registers -> wgmma m64 x BN (B = the W planes, shared-memory descriptors), fp32
+//                    accumulators in registers; then the epilogue straight from the accumulators
+//   warp 8           TMA producer: A [128 x BK] (fp32) and the W planes [BN x 128 B] into a STAGES-deep ring
+// The tile schedule is static: with `persistent` one CTA per SM walks the tiles (the producer fills the ring for the
+// next tile under the epilogue of the current one), otherwise one tile per CTA.  Both issue the same instructions per
+// tile, so their results are bit-identical.
+#include <cstring>
+#include <map>
+#include <mutex>
+#include <tuple>
+#include <cuda_fp16.h>
 #include "common.cuh"
 #include "kernels.cuh"
 #include "tc_common.cuh"
 
-#include <map>
-#include <mutex>
-#include <tuple>
-
 namespace {
 
-constexpr int BM = 128, BK = 32;
-constexpr int NTHREADS = 192;
+constexpr int BM = 128;
+constexpr int NTHREADS = 288;
+constexpr int PRODUCER_WARP = 8;
+enum { W_RAW = 0, W_TF32 = 1, W_F16 = 2 };
 
-struct GemmTcArgs {
+template <int BN, int NPASS, int WM>
+struct Cfg {
+  static constexpr int BK = WM == W_F16 ? 64 : 32;            // one 128-byte swizzle row of W per k-block
+  static constexpr int A_BYTES = BM * BK * 4;                 // raw fp32 A: one or two [128 x 32] boxes
+  static constexpr int W_PLANE = BN * 128;
+  static constexpr int PLANES = NPASS == 3 ? 2 : 1;
+  static constexpr int STAGE_BYTES = A_BYTES + PLANES * W_PLANE;
+  static constexpr int TMA_BYTES = A_BYTES + (WM == W_RAW ? 1 : PLANES) * W_PLANE;
+  static constexpr int STAGES = (196608 / STAGE_BYTES) < 6 ? (196608 / STAGE_BYTES) : 6;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+};
+
+struct GArgs {
   const float* bias;
   const float* R; int ldr;
   float* C; int ldc;
   int M, N, K, K1;
   float alpha;
   int relu;
-  // optional transposed output for columns >= vt_col0: VT[(m / n_pad), n - vt_col0, m % n_pad]
+  // optional transposed output for columns >= vt_col0: VT[(m / n_pad), n - vt_col0, m % n_pad] (V^T of the QKV
+  // projection for the tf32 attention kernel), with its tf32 lo plane in VTLO
   float* VT; int vt_col0; int n_pad;
-  // optional tf32 hi/lo planes for the attention operands (3xTF32 mode): columns [256,512) (= K) are
-  // stored as rn_tf32 in C with the remainder in KLO [M,256]; V^T likewise in VT / VTLO
+  // tf32 planes of the attention's K operand: columns [256,512) are stored as rn_tf32 in C, the remainder in KLO [M,256]
   float* KLO; float* VTLO;
+  // half-precision operand planes for attention_h3.cu (fp16x3): K hi / lo and V hi / lo, all [rows, 256] (V stays
+  // key-major: the attention reads it as an MN-major B operand); when set they replace the fp32 K and V thirds of C
+  __half* KH16; __half* KL16; __half* VH16; __half* VL16;
+  int tiles_m, tiles_n;
+  // split-K (weight-gradient GEMMs: few output tiles, a very long contraction): K is cut into `ksplit` slices, slice s
+  // writes its partial product to rows [s * tiles_m * BM, ...) of C (a slab buffer that a small kernel sums afterwards,
+  // in fixed order).  1 = off.
+  int ksplit;
 };
 
-template <int BN, int NPASS>
-struct Cfg {
-  static constexpr int STAGES = (BN == 256) ? (NPASS == 3 ? 2 : 4) : (NPASS == 3 ? 3 : 4);
-  static constexpr int A_BYTES = BM * BK * 4;
-  static constexpr int W_BYTES = BN * BK * 4;
-  static constexpr int STAGE_BYTES = (A_BYTES + W_BYTES) * (NPASS == 3 ? 2 : 1);
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+// SCORE mode: one launch computes every (pair, tuple) score matrix  scores = mdesc_a . mdesc_b^T * alpha  into the
+// inner [m, n] block of the [m+1, n+1] coupling buffers.  A = descriptors of view a (raw fp32, split on chip), W = the
+// tf32 planes of the descriptors of view b.
+struct ScoreTab {
+  int n_pairs, batch, n_views, n_pad;
+  int a[MVM_MAX_PAIRS], b[MVM_MAX_PAIRS], m[MVM_MAX_PAIRS], n[MVM_MAX_PAIRS];
+  float* scores[MVM_MAX_PAIRS];
 };
 
-template <int BN, int NPASS, bool PRE>
+// rn_tf32 of a finite value (ties away, == cvt.rna.tf32.f32) in two integer instructions
+__device__ __forceinline__ float tf32_hi(float x) {
+  return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
+}
+__device__ __forceinline__ void split_pack_h(float x0, float x1, uint32_t& hi, uint32_t& lo) {
+  const __half2 h = __floats2half2_rn(x0, x1);
+  const float2 hf = __half22float2(h);
+  const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+
+template <int BN, int NPASS, int WM, bool SCORE>
 __global__ void __launch_bounds__(NTHREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-               const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmWlo, GemmTcArgs g) {
-  using C_ = Cfg<BN, NPASS>;
+gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
+               const __grid_constant__ CUtensorMap tmWhi, const __grid_constant__ CUtensorMap tmWlo,
+               const __grid_constant__ GArgs g, const __grid_constant__ ScoreTab st) {
+  using C_ = Cfg<BN, NPASS, WM>;
+  static_assert(NPASS == 3 || WM == W_RAW, "single pass reads the raw W");
+  constexpr int BK = C_::BK, STAGES = C_::STAGES, A_BYTES = C_::A_BYTES, W_PLANE = C_::W_PLANE;
+  constexpr int STAGE_BYTES = C_::STAGE_BYTES;
+  constexpr int KSTEPS = 4;                                   // 4 x (K = 8 tf32 | K = 16 halves) per k-block
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_::STAGES * C_::STAGE_BYTES);
-  uint64_t* full = bars;                       // TMA landed
-  uint64_t* empty = bars + C_::STAGES;         // MMAs that read the slot retired
-  uint64_t* split = bars + 2 * C_::STAGES;     // lo planes written (NPASS == 3)
-  uint64_t* tmem_full = bars + 3 * C_::STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * C_::STAGES + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);   // [STAGES] TMA landed
+  uint64_t* empty = full + STAGES;                                              // [STAGES] both warpgroups done (256)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int nk = g.K / BK;
-
-  auto stage_A = [&](int s) { return smem + s * C_::STAGE_BYTES; };
-  auto stage_W = [&](int s) { return smem + s * C_::STAGE_BYTES + C_::A_BYTES; };
-  auto stage_Alo = [&](int s) { return smem + s * C_::STAGE_BYTES + C_::A_BYTES + C_::W_BYTES; };
-  auto stage_Wlo = [&](int s) { return smem + s * C_::STAGE_BYTES + 2 * C_::A_BYTES + C_::W_BYTES; };
+  const int nk = SCORE ? g.K / BK : g.K / BK / g.ksplit;     // k-blocks per tile (per K slice)
+  const int per_prob = g.tiles_m * g.tiles_n;
+  const int n_tiles = SCORE ? per_prob * st.n_pairs * st.batch : per_prob * g.ksplit;
+  // tile -> output tile origin (m0, n0), the rows the A / W boxes start at, and the problem (K slice or pair x tuple)
+  auto decode = [&](int tile, int& m0, int& n0, int& a_row, int& w_row, int& prob) {
+    prob = tile / per_prob;
+    const int r = tile % per_prob;
+    m0 = (r / g.tiles_n) * BM; n0 = (r % g.tiles_n) * BN;
+    if (!SCORE) {
+      a_row = m0; w_row = n0;
+    } else {
+      const int p = prob / st.batch, bi = prob % st.batch;
+      a_row = (bi * st.n_views + st.a[p]) * st.n_pad + m0;
+      w_row = (bi * st.n_views + st.b[p]) * st.n_pad + n0;
+    }
+  };
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < C_::STAGES; ++s) {
+    for (int s = 0; s < STAGES; ++s) {
       tc::mbar_init(full + s, 1);
-      tc::mbar_init(empty + s, 1);
-      tc::mbar_init(split + s, 128);
+      tc::mbar_init(empty + s, 256);
     }
-    tc::mbar_init(tmem_full, 1);
     tc::fence_barrier_init();
   }
-  if (warp == 0 && lane == 0) {
-    tc::prefetch_tmap(&tmA);
-    tc::prefetch_tmap(&tmA2);
-    tc::prefetch_tmap(&tmW);
-  }
-  if (warp == 1) tc::tmem_alloc<BN>(tmem_slot);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ================================ TMA producer ================================
-    for (int kt = 0; kt < nk; ++kt) {
-      const int s = kt % C_::STAGES;
-      const uint32_t ph = (kt / C_::STAGES) & 1;
-      tc::mbar_wait(empty + s, ph ^ 1);
-      if (tc::elect_one()) {
-        tc::mbar_arrive_expect_tx(full + s, C_::A_BYTES + C_::W_BYTES * (PRE ? 2 : 1));
-        const int k = kt * BK;
-        if (k < g.K1) tc::tma_load_2d(stage_A(s), &tmA, full + s, k, m0);
-        else tc::tma_load_2d(stage_A(s), &tmA2, full + s, k - g.K1, m0);
-        tc::tma_load_2d(stage_W(s), &tmW, full + s, k, n0);            // PRE: the rn_tf32 plane of W
-        if (PRE) tc::tma_load_2d(stage_Wlo(s), &tmWlo, full + s, k, n0);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ================================
-    // converged warp, one elected lane issues (see tc::elect_one)
-    constexpr uint32_t idesc = tc::make_idesc_tf32(BM, BN);
-    for (int kt = 0; kt < nk; ++kt) {
-      const int s = kt % C_::STAGES;
-      const uint32_t ph = (kt / C_::STAGES) & 1;
-      tc::mbar_wait(full + s, ph);
-      if (NPASS == 3) tc::mbar_wait(split + s, ph);
-      tc::tc_fence_after();
-      const uint32_t a = tc::smem_u32(stage_A(s)), w = tc::smem_u32(stage_W(s));
-      const uint32_t alo = tc::smem_u32(stage_Alo(s)), wlo = tc::smem_u32(stage_Wlo(s));
-      if (tc::elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < BK / 8; ++kk) {
-          const uint32_t off = kk * 32;   // 8 tf32 = 32 bytes along K inside the 128B swizzle span
-          const uint64_t da = tc::make_kmajor_sw128_desc(a + off), dw = tc::make_kmajor_sw128_desc(w + off);
-          tc::umma_tf32(tmem_base, da, dw, idesc, (kt | kk) != 0);
-          if (NPASS == 3) {
-            tc::umma_tf32(tmem_base, da, tc::make_kmajor_sw128_desc(wlo + off), idesc, 1);
-            tc::umma_tf32(tmem_base, tc::make_kmajor_sw128_desc(alo + off), dw, idesc, 1);
+    if (lane == 0) {
+      tc::prefetch_tmap(&tmA); tc::prefetch_tmap(&tmA2); tc::prefetch_tmap(&tmWhi); tc::prefetch_tmap(&tmWlo);
+      uint32_t it = 0;
+      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        int m0, n0, a_row, w_row, prob;
+        decode(tile, m0, n0, a_row, w_row, prob);
+        for (int kt = 0; kt < nk; ++kt, ++it) {
+          const int s = it % STAGES;
+          tc::mbar_wait(empty + s, ((it / STAGES) & 1) ^ 1);
+          tc::mbar_arrive_expect_tx(full + s, C_::TMA_BYTES);
+          uint8_t* sp = smem + s * STAGE_BYTES;
+          const int k = kt * BK + (SCORE ? 0 : prob * nk * BK);
+          if (k < g.K1) tc::tma_load_2d(sp, &tmA, full + s, k, a_row);
+          else tc::tma_load_2d(sp, &tmA2, full + s, k - g.K1, a_row);
+          if (WM == W_F16) {   // second [128 x 32] fp32 box of the 64-wide k-block (K1 is a multiple of 64)
+            if (k < g.K1) tc::tma_load_2d(sp + 16384, &tmA, full + s, k + 32, a_row);
+            else tc::tma_load_2d(sp + 16384, &tmA2, full + s, k + 32 - g.K1, a_row);
           }
+          tc::tma_load_2d(sp + A_BYTES, &tmWhi, full + s, k, w_row);
+          if (WM != W_RAW) tc::tma_load_2d(sp + A_BYTES + W_PLANE, &tmWlo, full + s, k, w_row);
         }
-        tc::umma_commit(empty + s);
-        if (kt == nk - 1) tc::umma_commit(tmem_full);
       }
-      __syncwarp();
     }
-  } else {
-    // ================================ splitters, then epilogue ================================
-    const int et = threadIdx.x - 64;   // 0..127
-    if (NPASS == 3) {
-      for (int kt = 0; kt < nk; ++kt) {
-        const int s = kt % C_::STAGES;
-        const uint32_t ph = (kt / C_::STAGES) & 1;
-        tc::mbar_wait(full + s, ph);
-        // lo planes are element-wise images of the landed tiles: same (swizzled) offsets
-        // hi = rn_tf32(x) replaces the landed tile in place, lo = rn_tf32(x - hi) goes to the second
-        // buffer; both are element-wise images of the tile, so the (swizzled) offsets carry over
-        float4* a = reinterpret_cast<float4*>(stage_A(s));
-        float4* alo = reinterpret_cast<float4*>(stage_Alo(s));
+    return;
+  }
+
+  // ================================ consumers ================================
+  const int wg = warp >> 2, wq = warp & 3;
+  const int gr = lane >> 2, tq = lane & 3;
+  const int row0 = wg * 64 + wq * 16 + gr;                     // tile rows of this thread: row0, row0 + 8
+  float acc[BN / 2];
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    int m0, n0, a_row, w_row, prob;
+    decode(tile, m0, n0, a_row, w_row, prob);
 #pragma unroll
-        for (int i = 0; i < (BM * BK / 4) / 128; ++i) {
-          const float4 x = a[et + i * 128];
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kt = 0; kt < nk; ++kt, ++it) {
+      const int s = it % STAGES;
+      tc::mbar_wait(full + s, (it / STAGES) & 1);
+      uint8_t* sp = smem + s * STAGE_BYTES;
+      if (WM == W_RAW && NPASS == 3) {
+        // hi = rn_tf32(w) replaces the landed tile in place, lo = rn_tf32(w - hi) goes to the second plane; both are
+        // element-wise images of the tile, so the (swizzled) offsets carry over
+        float4* w = reinterpret_cast<float4*>(sp + A_BYTES);
+        float4* wl = reinterpret_cast<float4*>(sp + A_BYTES + W_PLANE);
+#pragma unroll 4
+        for (int i = threadIdx.x; i < BN * 32 / 4; i += 256) {
+          const float4 x = w[i];
           float4 h;
           h.x = tc::tf32_rn(x.x); h.y = tc::tf32_rn(x.y); h.z = tc::tf32_rn(x.z); h.w = tc::tf32_rn(x.w);
-          a[et + i * 128] = h;
-          alo[et + i * 128] = make_float4(tc::tf32_rn(x.x - h.x), tc::tf32_rn(x.y - h.y), tc::tf32_rn(x.z - h.z),
-                                          tc::tf32_rn(x.w - h.w));
-        }
-        float4* w = reinterpret_cast<float4*>(stage_W(s));
-        float4* wlo = reinterpret_cast<float4*>(stage_Wlo(s));
-#pragma unroll
-        for (int i = 0; i < (PRE ? 0 : (BN * BK / 4) / 128); ++i) {
-          const float4 x = w[et + i * 128];
-          float4 h;
-          h.x = tc::tf32_rn(x.x); h.y = tc::tf32_rn(x.y); h.z = tc::tf32_rn(x.z); h.w = tc::tf32_rn(x.w);
-          w[et + i * 128] = h;
-          wlo[et + i * 128] = make_float4(tc::tf32_rn(x.x - h.x), tc::tf32_rn(x.y - h.y), tc::tf32_rn(x.z - h.z),
-                                          tc::tf32_rn(x.w - h.w));
+          w[i] = h;
+          wl[i] = make_float4(tc::tf32_rn(x.x - h.x), tc::tf32_rn(x.y - h.y), tc::tf32_rn(x.z - h.z), tc::tf32_rn(x.w - h.w));
         }
         tc::fence_proxy_async();      // generic-proxy writes -> visible to the tensor core (async proxy)
-        tc::mbar_arrive(split + s);
+        asm volatile("bar.sync 1, 256;" ::: "memory");
       }
-    }
-    tc::mbar_wait(tmem_full, 0);
-    tc::tc_fence_after();
-    const int q = warp & 3;                     // TMEM lane quarter this warp may read
-    const int row = q * 32 + lane;
-    const int m = m0 + row;
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    for (int c = 0; c < BN / 32; ++c) {
-      float v[32];
-      tc::tmem_ld32(taddr + c * 32, v);
-      tc::tmem_ld_wait();
-      if (m < g.M) {
-        const int nb = n0 + c * 32;
+      // A fragments of rows row0 / row0 + 8 from the 128B-swizzled tile: 16-byte chunk c of row r sits at c ^ (r & 7)
+      uint32_t ahi[KSTEPS][4], alo[KSTEPS][4];
+      const uint8_t* ar = sp + row0 * 128;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          float x = g.alpha * v[j];
-          if (g.bias) x += __ldg(g.bias + nb + j);
-          if (g.relu) x = fmaxf(x, 0.f);
-          v[j] = x;
-        }
-        if (g.R) {
-          const float4* r4 = reinterpret_cast<const float4*>(g.R + (long long)m * g.ldr + nb);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 r = r4[j];
-            v[4 * j] += r.x; v[4 * j + 1] += r.y; v[4 * j + 2] += r.z; v[4 * j + 3] += r.w;
-          }
-        }
-        if (g.VT && nb >= g.vt_col0) {
-          const int slab = m / g.n_pad, i = m % g.n_pad;
-          const long long off = ((long long)slab * (g.N - g.vt_col0) + (nb - g.vt_col0)) * g.n_pad + i;
-          if (g.VTLO) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float hi = tc::tf32_rn(v[j]);
-              g.VT[off + (long long)j * g.n_pad] = hi;
-              g.VTLO[off + (long long)j * g.n_pad] = tc::tf32_rn(v[j] - hi);
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) g.VT[off + (long long)j * g.n_pad] = v[j];
-          }
-        } else if (g.KLO && nb >= 256 && nb < 512) {
-          float4* o = reinterpret_cast<float4*>(g.C + (long long)m * g.ldc + nb);
-          float4* ol = reinterpret_cast<float4*>(g.KLO + (long long)m * 256 + (nb - 256));
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 h;
-            h.x = tc::tf32_rn(v[4 * j]); h.y = tc::tf32_rn(v[4 * j + 1]); h.z = tc::tf32_rn(v[4 * j + 2]); h.w = tc::tf32_rn(v[4 * j + 3]);
-            o[j] = h;
-            ol[j] = make_float4(tc::tf32_rn(v[4 * j] - h.x), tc::tf32_rn(v[4 * j + 1] - h.y), tc::tf32_rn(v[4 * j + 2] - h.z),
-                                tc::tf32_rn(v[4 * j + 3] - h.w));
-          }
+      for (int kk = 0; kk < KSTEPS; ++kk) {
+        if (WM == W_F16) {
+          const uint8_t* ab = ar + (kk >> 1) * 16384;
+          const int ch = 4 * (kk & 1) + (tq >> 1), wo = (tq & 1) * 8;
+          const float2 x0 = *reinterpret_cast<const float2*>(ab + ((ch ^ gr) << 4) + wo);
+          const float2 x1 = *reinterpret_cast<const float2*>(ab + 1024 + ((ch ^ gr) << 4) + wo);
+          const float2 x2 = *reinterpret_cast<const float2*>(ab + (((ch + 2) ^ gr) << 4) + wo);
+          const float2 x3 = *reinterpret_cast<const float2*>(ab + 1024 + (((ch + 2) ^ gr) << 4) + wo);
+          split_pack_h(x0.x, x0.y, ahi[kk][0], alo[kk][0]);
+          split_pack_h(x1.x, x1.y, ahi[kk][1], alo[kk][1]);
+          split_pack_h(x2.x, x2.y, ahi[kk][2], alo[kk][2]);
+          split_pack_h(x3.x, x3.y, ahi[kk][3], alo[kk][3]);
         } else {
-          float4* o = reinterpret_cast<float4*>(g.C + (long long)m * g.ldc + nb);
+          float x[4];
+          x[0] = *reinterpret_cast<const float*>(ar + (((2 * kk) ^ gr) << 4) + tq * 4);
+          x[1] = *reinterpret_cast<const float*>(ar + 1024 + (((2 * kk) ^ gr) << 4) + tq * 4);
+          x[2] = *reinterpret_cast<const float*>(ar + (((2 * kk + 1) ^ gr) << 4) + tq * 4);
+          x[3] = *reinterpret_cast<const float*>(ar + 1024 + (((2 * kk + 1) ^ gr) << 4) + tq * 4);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) o[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+          for (int e = 0; e < 4; ++e) {
+            if (NPASS == 3) {
+              const float h = tf32_hi(x[e]);
+              ahi[kk][e] = __float_as_uint(h);
+              alo[kk][e] = __float_as_uint(tf32_hi(x[e] - h));
+            } else {
+              ahi[kk][e] = __float_as_uint(x[e]);   // the tensor core reads the top 19 bits
+            }
+          }
+        }
+      }
+      const uint32_t whi = tc::smem_u32(sp + A_BYTES);
+      tc::wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < KSTEPS; ++kk) {
+#pragma unroll
+        for (int nh = 0; nh < BN / 128; ++nh) {
+          float* d = acc + nh * 64;
+          const uint32_t wb = whi + nh * 16384 + kk * 32;     // 32 bytes along K inside the 128-byte row
+          if (WM == W_F16) {
+            tc::wgmma_f16_rs<128, 0>(d, ahi[kk], tc::make_sw128_desc(wb));
+            tc::wgmma_f16_rs<128, 0>(d, ahi[kk], tc::make_sw128_desc(wb + W_PLANE));
+            tc::wgmma_f16_rs<128, 0>(d, alo[kk], tc::make_sw128_desc(wb));
+          } else {
+            tc::wgmma_tf32_rs<128>(d, ahi[kk], tc::make_sw128_desc(wb));
+            if (NPASS == 3) {
+              tc::wgmma_tf32_rs<128>(d, ahi[kk], tc::make_sw128_desc(wb + W_PLANE));
+              tc::wgmma_tf32_rs<128>(d, alo[kk], tc::make_sw128_desc(wb));
+            }
+          }
+        }
+      }
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      tc::fence_acc<BN>(acc);
+      tc::mbar_arrive(empty + s);
+    }
+
+    // ================================ epilogue ================================
+    if (SCORE) {
+      // rows of the coupling buffer are n+1 floats long: plain stores inside the [m, n] block
+      const int p = prob / st.batch, bi = prob % st.batch;
+      const int pm = st.m[p], pn = st.n[p];
+      float* Cp = st.scores[p] + (long long)bi * (pm + 1) * (pn + 1);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int gm = m0 + row0 + 8 * hh;
+        if (gm >= pm) continue;
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+          const int gn = n0 + 8 * i + 2 * tq;
+          if (gn < pn) Cp[(long long)gm * (pn + 1) + gn] = g.alpha * acc[4 * i + 2 * hh];
+          if (gn + 1 < pn) Cp[(long long)gm * (pn + 1) + gn + 1] = g.alpha * acc[4 * i + 2 * hh + 1];
+        }
+      }
+      continue;
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int m = m0 + row0 + 8 * hh;
+      if (m >= g.M) continue;
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) {
+        const int n = n0 + 8 * i + 2 * tq;
+        float x0 = g.alpha * acc[4 * i + 2 * hh], x1 = g.alpha * acc[4 * i + 2 * hh + 1];
+        if (g.bias) { x0 += __ldg(g.bias + n); x1 += __ldg(g.bias + n + 1); }
+        if (g.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        if (g.R) {
+          const float2 r = __ldg(reinterpret_cast<const float2*>(g.R + (long long)m * g.ldr + n));
+          x0 += r.x; x1 += r.y;
+        }
+        if (g.VT && n >= g.vt_col0) {
+          // V^T (and its tf32 lo plane) for the tf32 attention kernel
+          const int slab = m / g.n_pad, ii = m % g.n_pad;
+          const long long off = ((long long)slab * (g.N - g.vt_col0) + (n - g.vt_col0)) * g.n_pad + ii;
+          if (g.VTLO) {
+            const float h0 = tf32_hi(x0), h1 = tf32_hi(x1);
+            g.VT[off] = h0; g.VT[off + g.n_pad] = h1;
+            g.VTLO[off] = tf32_hi(x0 - h0); g.VTLO[off + g.n_pad] = tf32_hi(x1 - h1);
+          } else {
+            g.VT[off] = x0; g.VT[off + g.n_pad] = x1;
+          }
+        } else if (g.KH16 && n >= 256) {
+          // K (columns 256..511) and V (512..767) hi / lo planes in half precision
+          const bool is_v = n >= 512;
+          const long long o = (long long)m * 256 + n - (is_v ? 512 : 256);
+          uint32_t hi, lo;
+          split_pack_h(x0, x1, hi, lo);
+          *reinterpret_cast<uint32_t*>((is_v ? g.VH16 : g.KH16) + o) = hi;
+          *reinterpret_cast<uint32_t*>((is_v ? g.VL16 : g.KL16) + o) = lo;
+        } else if (g.KLO && n >= 256 && n < 512) {
+          const float h0 = tf32_hi(x0), h1 = tf32_hi(x1);
+          *reinterpret_cast<float2*>(g.C + (long long)m * g.ldc + n) = make_float2(h0, h1);
+          *reinterpret_cast<float2*>(g.KLO + (long long)m * 256 + n - 256) = make_float2(tf32_hi(x0 - h0), tf32_hi(x1 - h1));
+        } else {
+          const long long c_row = m + (long long)prob * g.tiles_m * BM;     // split-K: slab of this K slice
+          *reinterpret_cast<float2*>(g.C + c_row * g.ldc + n) = make_float2(x0, x1);
         }
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc<BN>(tmem_base);
+}
+
+template <int BN, int NPASS, int WM, bool SCORE>
+int launch_wg(const CUtensorMap* tA, const CUtensorMap* tA2, const CUtensorMap* tWhi, const CUtensorMap* tWlo,
+              const GArgs& g, const ScoreTab& st, long long n_tiles, bool persistent, cudaStream_t stream) {
+  using C_ = Cfg<BN, NPASS, WM>;
+  if (!tA || !tA2 || !tWhi || !tWlo) return MVM_ERR_LAUNCH;
+  if (n_tiles <= 0) return MVM_OK;
+  // cheap and idempotent: set on every launch (per-device attribute)
+  cudaFuncSetAttribute(gemm_wg_kernel<BN, NPASS, WM, SCORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES);
+  const int n_sm = mvm_dev_info().n_sm;
+  const int grid = (persistent && n_tiles > n_sm) ? n_sm : (int)n_tiles;
+  gemm_wg_kernel<BN, NPASS, WM, SCORE><<<grid, NTHREADS, C_::SMEM_BYTES, stream>>>(*tA, *tA2, *tWhi, *tWlo, g, st);
+  MVM_CHECK_LAUNCH();
+  return MVM_OK;
+}
+
+GArgs make_args(const GemmDesc& d, float* VT, int vt_col0, int n_pad, float* KLO, float* VTLO, int bn) {
+  GArgs g;
+  memset(&g, 0, sizeof(g));
+  g.bias = d.bias; g.R = d.R; g.ldr = d.ldr; g.C = d.C; g.ldc = d.ldc; g.M = d.M; g.N = d.N; g.K = d.K;
+  g.K1 = d.K1; g.alpha = d.alpha; g.relu = d.relu; g.VT = VT; g.vt_col0 = vt_col0; g.n_pad = n_pad;
+  g.KLO = KLO; g.VTLO = VTLO;
+  g.tiles_m = mvm_div_up(d.M, BM); g.tiles_n = d.N / bn; g.ksplit = 1;
+  return g;
+}
+
+ScoreTab no_scores() {
+  ScoreTab none;
+  memset(&none, 0, sizeof(none));
+  return none;
+}
+
+template <int BN, int NPASS, int WM>
+int launch_cfg(const GemmDesc& d, float* VT, int vt_col0, int n_pad, float* KLO, float* VTLO, bool persistent,
+               cudaStream_t stream) {
+  const CUtensorMap* tA = mvm_get_tmap_2d(d.A, d.M, d.K1, d.lda, BM);
+  const CUtensorMap* tA2 = d.A2 ? mvm_get_tmap_2d(d.A2, d.M, d.K - d.K1, d.lda2, BM) : tA;
+  const CUtensorMap* tW = mvm_get_tmap_2d(WM == W_TF32 ? d.Whi : d.W, d.N, d.K, d.ldw, BN);
+  const CUtensorMap* tWlo = WM == W_TF32 ? mvm_get_tmap_2d(d.Wlo, d.N, d.K, d.ldw, BN) : tW;
+  const GArgs g = make_args(d, VT, vt_col0, n_pad, KLO, VTLO, BN);
+  return launch_wg<BN, NPASS, WM, false>(tA, tA2, tW, tWlo, g, no_scores(), (long long)g.tiles_m * g.tiles_n, persistent,
+                                         stream);
+}
+
+
+// hi = rn_tf32(x), lo = rn_tf32(x - hi) of a whole buffer (the W-operand planes of the score GEMM)
+__global__ void split_planes_kernel(const float4* __restrict__ x, float4* __restrict__ hi, float4* __restrict__ lo,
+                                    long long n4) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    const float4 v = x[i];
+    float4 h, l;
+    h.x = tf32_hi(v.x); h.y = tf32_hi(v.y); h.z = tf32_hi(v.z); h.w = tf32_hi(v.w);
+    l.x = tf32_hi(v.x - h.x); l.y = tf32_hi(v.y - h.y); l.z = tf32_hi(v.z - h.z); l.w = tf32_hi(v.w - h.w);
+    hi[i] = h;
+    lo[i] = l;
+  }
+}
+
+// C[m, n] = sum_s slabs[s][m][n] (fixed order: deterministic)
+__global__ void splitk_reduce_kernel(const float4* __restrict__ slabs, float* __restrict__ C, int M, int N4, int ldc, int S) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= (long long)M * N4) return;
+  const int m = (int)(i / N4), n4 = (int)(i % N4);
+  float4 a = slabs[i];
+  for (int s = 1; s < S; ++s) {
+    const float4 b = slabs[(long long)s * M * N4 + i];
+    a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+  }
+  *reinterpret_cast<float4*>(C + (long long)m * ldc + 4 * n4) = a;
 }
 
 // ---- host: tensor-map cache -------------------------------------------------------------------
@@ -254,25 +404,6 @@ EncodeFn get_encode() {
 typedef std::tuple<const void*, long long, long long, long long, long long, long long, int> TmKey;
 std::map<TmKey, CUtensorMap*> g_tmaps;
 std::mutex g_tmap_mu;
-
-template <int BN, int NPASS, bool PRE>
-int launch_cfg(const GemmDesc& d, float* VT, int vt_col0, int n_pad, float* KLO, float* VTLO, cudaStream_t stream) {
-  using C_ = Cfg<BN, NPASS>;
-  // cheap and idempotent: set on every launch (per-device attribute; 12 template instances)
-  cudaFuncSetAttribute(gemm_tc_kernel<BN, NPASS, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES);
-  const CUtensorMap* tA = mvm_get_tmap_2d(d.A, d.M, d.K1, d.lda, BM);
-  const CUtensorMap* tA2 = d.A2 ? mvm_get_tmap_2d(d.A2, d.M, d.K - d.K1, d.lda2, BM) : tA;
-  const CUtensorMap* tW = mvm_get_tmap_2d(PRE ? d.Whi : d.W, d.N, d.K, d.ldw, BN);
-  const CUtensorMap* tWlo = PRE ? mvm_get_tmap_2d(d.Wlo, d.N, d.K, d.ldw, BN) : tW;
-  if (!tA || !tA2 || !tW || !tWlo) return MVM_ERR_LAUNCH;
-  GemmTcArgs g;
-  g.bias = d.bias; g.R = d.R; g.ldr = d.ldr; g.C = d.C; g.ldc = d.ldc; g.M = d.M; g.N = d.N; g.K = d.K;
-  g.K1 = d.K1; g.alpha = d.alpha; g.relu = d.relu; g.VT = VT; g.vt_col0 = vt_col0; g.n_pad = n_pad; g.KLO = KLO; g.VTLO = VTLO;
-  dim3 grid(d.N / BN, mvm_div_up(d.M, BM));
-  gemm_tc_kernel<BN, NPASS, PRE><<<grid, NTHREADS, C_::SMEM_BYTES, stream>>>(*tA, *tA2, *tW, *tWlo, g);
-  MVM_CHECK_LAUNCH();
-  return MVM_OK;
-}
 
 }  // namespace
 
@@ -331,35 +462,10 @@ const CUtensorMap* mvm_get_tmap_2d_f16(const void* base, long long rows, long lo
   return tm;
 }
 
-// 2-D fp16 row-major [rows, cols] STORE map of the persistent GEMM's plane epilogue: box = [32 rows, 32 cols = 64 B],
-// 64-byte swizzle (a warp stages 32 rows x 64 B conflict-free and one TMA store writes them as full lines)
-const CUtensorMap* mvm_get_tmap_2d_f16_store(const void* base, long long rows, long long cols, long long ld) {
-  std::lock_guard<std::mutex> lk(g_tmap_mu);
-  TmKey key(base, -17, rows, cols, ld, 0, 32);
-  auto it = g_tmaps.find(key);
-  if (it != g_tmaps.end()) return it->second;
-  EncodeFn enc = get_encode();
-  if (!enc) return nullptr;
-  CUtensorMap* tm = new CUtensorMap;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {32, 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    fprintf(stderr, "[mvm_b200] cuTensorMapEncodeTiled (f16 store) failed (%d) rows=%lld cols=%lld ld=%lld\n", (int)r, rows, cols, ld);
-    delete tm;
-    return nullptr;
-  }
-  g_tmaps[key] = tm;
-  return tm;
-}
 
-int g_gemm_bn = 256;   // output tile width of the one-tile-per-CTA tcgen05 GEMM (128 or 256), see mvm_debug_set_gemm_tile
+int g_gemm_bn = 256;   // output tile width of the one-tile-per-CTA schedule (128 or 256), see mvm_debug_set_gemm_tile
 extern "C" void mvm_debug_set_gemm_tile(int bn) { g_gemm_bn = bn == 256 ? 256 : 128; }
-int g_gemm_persist = 1;   // 1: the persistent kernel of gemm_tc_persist.cu serves the 3xTF32 path (default)
+int g_gemm_persist = 1;   // 1: the persistent schedule with pre-split W planes serves the 3xTF32 path (default)
 extern "C" void mvm_debug_set_gemm_kernel(int persistent) { g_gemm_persist = persistent ? 1 : 0; }
 
 // GEMM on the tensor cores.  Requirements: K, K1 multiples of 32, N multiple of 128, 16-byte aligned
@@ -371,16 +477,82 @@ int launch_gemm_tc(const GemmDesc& d, int n_pass, float* VT, int vt_col0, int n_
                    float* KLO, float* VTLO, int gemm_tile, int gemm_persist) {
   if (gemm_tile < 0) gemm_tile = g_gemm_bn;            // stage-level callers: the process defaults
   if (gemm_persist < 0) gemm_persist = g_gemm_persist;
-  MVM_REQUIRE(d.batch == 1 && d.K % BK == 0 && d.K1 % BK == 0 && d.N % 128 == 0);
+  MVM_REQUIRE(d.batch == 1 && d.K % 32 == 0 && d.K1 % 32 == 0 && d.N % 128 == 0);
   MVM_REQUIRE(d.lda % 4 == 0 && d.ldw % 4 == 0 && d.ldc % 4 == 0 && (d.R == nullptr || d.ldr % 4 == 0));
   MVM_REQUIRE(d.A2 == nullptr || d.lda2 % 4 == 0);
   MvmProfScope prof__(MVM_TAG_GEMM, stream);
   if (gemm_persist && n_pass == 3 && d.Whi && d.Wlo) return launch_gemm_tc_persist(d, VT, vt_col0, n_pad, KLO, VTLO, stream);
   if (gemm_tile == 256 && d.N % 256 == 0) {
-    if (n_pass == 3 && d.Whi && d.Wlo) return launch_cfg<256, 3, true>(d, VT, vt_col0, n_pad, KLO, VTLO, stream);
-    if (n_pass == 1) return launch_cfg<256, 1, false>(d, VT, vt_col0, n_pad, nullptr, nullptr, stream);
+    if (n_pass == 3 && d.Whi && d.Wlo) return launch_cfg<256, 3, W_TF32>(d, VT, vt_col0, n_pad, KLO, VTLO, false, stream);
+    if (n_pass == 1) return launch_cfg<256, 1, W_RAW>(d, VT, vt_col0, n_pad, nullptr, nullptr, false, stream);
   }
-  if (n_pass == 3 && d.Whi && d.Wlo) return launch_cfg<128, 3, true>(d, VT, vt_col0, n_pad, KLO, VTLO, stream);
-  if (n_pass == 3) return launch_cfg<128, 3, false>(d, VT, vt_col0, n_pad, KLO, VTLO, stream);
-  return launch_cfg<128, 1, false>(d, VT, vt_col0, n_pad, nullptr, nullptr, stream);
+  if (n_pass == 3 && d.Whi && d.Wlo) return launch_cfg<128, 3, W_TF32>(d, VT, vt_col0, n_pad, KLO, VTLO, false, stream);
+  if (n_pass == 3) return launch_cfg<128, 3, W_RAW>(d, VT, vt_col0, n_pad, KLO, VTLO, false, stream);
+  return launch_cfg<128, 1, W_RAW>(d, VT, vt_col0, n_pad, nullptr, nullptr, false, stream);
+}
+
+// Persistent schedule, 128-column tiles, W given as its tf32 planes or (fp16x3) as half-precision planes of
+// wscale * W.  Requirements as launch_gemm_tc; the fp16 planes are used when given and K, K1 are multiples of 64.
+int launch_gemm_tc_persist(const GemmDesc& d, float* VT, int vt_col0, int n_pad, float* KLO, float* VTLO,
+                           cudaStream_t stream, const HalfPlanes* hp, int ksplit, float* slabs) {
+  // split-K: partial products of the K slices go to slabs [ksplit, M, N] (M a multiple of the tile height), summed by
+  // launch_splitk_reduce afterwards; no bias / residual / activation / concat in that mode
+  MVM_REQUIRE(ksplit >= 1 && (ksplit == 1 || (slabs && d.M % BM == 0 && d.K % (32 * ksplit) == 0 && !d.Whi16 && !d.bias && !d.R && !d.A2 &&
+                                               !d.relu && !VT && !KLO && !hp)));
+  const bool f16 = d.Whi16 != nullptr && d.Wlo16 != nullptr && d.K % 64 == 0 && d.K1 % 64 == 0 && d.wscale > 0.f;
+  const CUtensorMap* tA = mvm_get_tmap_2d(d.A, d.M, d.K1, d.lda, BM);
+  const CUtensorMap* tA2 = d.A2 ? mvm_get_tmap_2d(d.A2, d.M, d.K - d.K1, d.lda2, BM) : tA;
+  GArgs g = make_args(d, VT, vt_col0, n_pad, KLO, VTLO, 128);
+  if (ksplit > 1) { g.C = slabs; g.ldc = d.N; }
+  g.ksplit = ksplit;
+  if (hp) {
+    g.KH16 = (__half*)hp->kh; g.KL16 = (__half*)hp->kl; g.VH16 = (__half*)hp->vh; g.VL16 = (__half*)hp->vl;
+  }
+  const long long n_tiles = (long long)g.tiles_m * g.tiles_n * ksplit;
+  if (f16) {
+    g.alpha = d.alpha / d.wscale;
+    const CUtensorMap* tWhi = mvm_get_tmap_2d_f16(d.Whi16, d.N, d.K, d.ldw, 128);
+    const CUtensorMap* tWlo = mvm_get_tmap_2d_f16(d.Wlo16, d.N, d.K, d.ldw, 128);
+    return launch_wg<128, 3, W_F16, false>(tA, tA2, tWhi, tWlo, g, no_scores(), n_tiles, true, stream);
+  }
+  const CUtensorMap* tWhi = mvm_get_tmap_2d(d.Whi, d.N, d.K, d.ldw, 128);
+  const CUtensorMap* tWlo = mvm_get_tmap_2d(d.Wlo, d.N, d.K, d.ldw, 128);
+  return launch_wg<128, 3, W_TF32, false>(tA, tA2, tWhi, tWlo, g, no_scores(), n_tiles, true, stream);
+}
+
+int launch_splitk_reduce(const float* slabs, float* C, int M, int N, int ldc, int ksplit, cudaStream_t stream) {
+  MVM_REQUIRE(N % 4 == 0 && ldc % 4 == 0);
+  const long long n = (long long)M * (N / 4);
+  splitk_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(slabs), C, M, N / 4, ldc, ksplit);
+  MVM_CHECK_LAUNCH();
+  return MVM_OK;
+}
+
+// All (pair, tuple) score matrices on the tensor cores (3xTF32).  mdesc [rows_total, 256] point-major; hi / lo:
+// scratch planes of the same size (filled here).
+int launch_score_gemm_tc(const float* mdesc, float* hi, float* lo, int n_pad, const PairTable& tab, int batch,
+                         float alpha, cudaStream_t stream) {
+  MvmProfScope prof__(MVM_TAG_SCORE, stream);
+  const int n_sm = mvm_dev_info().n_sm;
+  const long long rows = (long long)batch * tab.n_views * n_pad;
+  split_planes_kernel<<<n_sm * 4, 256, 0, stream>>>(reinterpret_cast<const float4*>(mdesc), reinterpret_cast<float4*>(hi),
+                                                    reinterpret_cast<float4*>(lo), rows * 256 / 4);
+  MVM_CHECK_LAUNCH();
+  const CUtensorMap* tA = mvm_get_tmap_2d(mdesc, rows, 256, 256, BM);
+  const CUtensorMap* tWhi = mvm_get_tmap_2d(hi, rows, 256, 256, 128);
+  const CUtensorMap* tWlo = mvm_get_tmap_2d(lo, rows, 256, 256, 128);
+  ScoreTab st = no_scores();
+  st.n_pairs = tab.n_pairs; st.batch = batch; st.n_views = tab.n_views; st.n_pad = n_pad;
+  int max_m = 0, max_n = 0;
+  for (int p = 0; p < tab.n_pairs; ++p) {
+    st.a[p] = tab.a[p]; st.b[p] = tab.b[p]; st.m[p] = tab.m[p]; st.n[p] = tab.n[p]; st.scores[p] = tab.scores[p];
+    max_m = tab.m[p] > max_m ? tab.m[p] : max_m;
+    max_n = tab.n[p] > max_n ? tab.n[p] : max_n;
+  }
+  GArgs g;
+  memset(&g, 0, sizeof(g));
+  g.K = 256; g.K1 = 256; g.alpha = alpha; g.ksplit = 1;
+  g.tiles_m = mvm_div_up(max_m, BM); g.tiles_n = mvm_div_up(max_n, 128);
+  const long long n_tiles = (long long)g.tiles_m * g.tiles_n * tab.n_pairs * batch;
+  return launch_wg<128, 3, W_TF32, true>(tA, tA, tWhi, tWlo, g, st, n_tiles, true, stream);
 }

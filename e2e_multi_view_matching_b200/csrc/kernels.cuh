@@ -28,20 +28,20 @@ int launch_kenc_front(const float* kpts, const float* kscores, const float* cons
 int launch_transpose_cn(const float* in, float* out, int n_views_total, int C, int n_pad,
                         cudaStream_t stream);
 
-// tcgen05 GEMM (gemm_tc.cu): n_pass 3 = fp32-faithful 3xTF32, 1 = single-pass TF32
+// tensor-core GEMM (gemm_tc.cu): n_pass 3 = fp32-faithful 3xTF32, 1 = single-pass TF32
 // gemm_tile (128 / 256) and gemm_persist (0 / 1) select the kernel; -1 = the process defaults
 int launch_gemm_tc(const GemmDesc& d, int n_pass, float* VT, int vt_col0, int n_pad, cudaStream_t stream,
                    float* KLO = nullptr, float* VTLO = nullptr, int gemm_tile = -1, int gemm_persist = -1);
 int mvm_default_gemm_tile();
 int mvm_default_gemm_persistent();
-// persistent 3xTF32 kernel (A operand in tensor memory, double-buffered accumulators, TMA-store epilogue)
+// persistent schedule of the same kernel with pre-split W planes (tf32, or fp16 when d.Whi16 / d.Wlo16 are given)
 // hp != nullptr (QKV projection, vt_col0 = 512): the K third and V^T leave as half-precision hi / lo planes for
 // launch_attention_h3 instead of the fp32 / tf32 buffers (kh, kl, vh, vl: all [rows, 256], as __half; V stays key-major)
 struct HalfPlanes { void* kh; void* kl; void* vh; void* vl; };
 int launch_gemm_tc_persist(const GemmDesc& d, float* VT, int vt_col0, int n_pad, float* KLO, float* VTLO,
                            cudaStream_t stream, const HalfPlanes* hp = nullptr, int ksplit = 1, float* slabs = nullptr);
 int launch_splitk_reduce(const float* slabs, float* C, int M, int N, int ldc, int ksplit, cudaStream_t stream);
-// every (pair, tuple) score matrix in one launch of the persistent kernel (3xTF32); hi / lo: scratch [rows, 256]
+// every (pair, tuple) score matrix in one launch of the GEMM kernel (3xTF32); hi / lo: scratch [rows, 256]
 struct PairTable;
 int launch_score_gemm_tc(const float* mdesc, float* hi, float* lo, int n_pad, const PairTable& tab, int batch,
                          float alpha, cudaStream_t stream);

@@ -69,7 +69,7 @@ GemmDesc make_gemm(const float* A, int lda, const float* W, int K, const float* 
 // PROCESS DEFAULTS of the per-call options (mvm_matcher_options).  They are read once, at the top of
 // mvm_matcher_forward, to fill the options of that call; nothing below this point reads or writes a global,
 // so two models / two streams / two threads may run forwards concurrently (each with its own workspace).
-// math mode: 3 = tcgen05 3xTF32 (fp32-faithful, DEFAULT), 1 = tcgen05 single-pass TF32, 0 = fp32 CUDA cores
+// math mode: 3 = 3xTF32 on the tensor cores (fp32-faithful, DEFAULT), 1 = single-pass TF32, 0 = fp32 CUDA cores
 int g_math_mode = 3;
 int g_score_tc = 1;                     // score GEMM on the tensor cores in mode 3 (mvm_debug_set_score_kernel)
 int g_gemm_split = 1;                   // operand planes of the mode-3 GEMMs: 1 = fp16 hi/lo (default, needs the packed half planes), 0 = tf32
@@ -137,7 +137,7 @@ void mvm_debug_set_score_kernel(int tc) { g_score_tc = tc ? 1 : 0; }
 void mvm_debug_set_attention_split(int fp16) { g_attn_split = fp16 ? 1 : 0; }
 void mvm_debug_set_gemm_split(int fp16) { g_gemm_split = fp16 ? 1 : 0; }
 
-const char* mvm_version(void) { return "mvm_b200 0.1 sm_100a"; }
+const char* mvm_version(void) { return "mvm_b200 0.1 sm_90a"; }
 
 size_t mvm_matcher_workspace_bytes(int batch, int n_views, int n_pad, int n_pairs, int has_conf) {
   return carve(nullptr, batch, n_views, n_pad, n_pairs, has_conf).total;

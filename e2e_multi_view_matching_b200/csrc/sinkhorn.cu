@@ -297,7 +297,7 @@ int launch_sinkhorn_log(const SinkhornTable& tab, int batch, float bin_score, in
 }
 
 size_t sinkhorn_ws_floats(int n_pairs, int batch, int n_pad) {
-  // counters + worst-case exchange ((2G+1)(n+1) per group, G*NG <= 148) and the v1 (u,v) scratch
+  // counters + worst-case exchange ((2G+1)(n+1) per group, G*NG <= the SM count) and the v1 (u,v) scratch
   // (sized for up to 192 SMs; the launchers check the real SM count against this bound)
   const size_t xch = 256 + (size_t)(2 * 192 + 192) * (n_pad + 1) * 2;   // log-domain partials / 8-byte LL words
   const size_t uv = (size_t)n_pairs * batch * (2 * (size_t)n_pad + 2);

@@ -3,12 +3,12 @@
 // sampling), so that eval_pairs / eval_multi_view go image-in -> pose-out on the device.
 //
 // Layout: activations NHWC fp32 (channels innermost: a warp's 32 pixels x one channel chunk are contiguous loads,
-// the 1x1 convolutions are plain row-major GEMMs on the tcgen05 kernel).  Weights are repacked on the host to
+// the 1x1 convolutions are plain row-major GEMMs on the tensor-core kernel).  Weights are repacked on the host to
 // [tap][Cin][Cout].
 //   sp_conv3x3_kernel     3x3 / pad 1 convolution + bias + ReLU, fp32 CUDA cores: a CTA computes 16 x 16 pixels x 32
 //                         output channels, input patch and weights staged in shared memory per 16-channel slice,
 //                         2 pixels x 32 channels of accumulators per thread.  (First cut of this row: an implicit-GEMM
-//                         tcgen05 version is the next step; the 1x1 heads already run on the tensor cores.)
+//                         tensor-core version is the next step; the 1x1 heads already run on the tensor cores.)
 //   sp_maxpool2_kernel    2x2 / stride 2 max pooling
 //   sp_scores_kernel      convPb (1x1, 256 -> 65) + softmax over the 65 bins + depth-to-space into the [8h, 8w] score map
 //   sp_maxpool_rows/cols  separable (2r+1)^2 max filter used by simple_nms (superpoint.py:47-63)
@@ -260,14 +260,14 @@ int conv3x3(const float* in, const float* w, const float* b, float* out, int B, 
   return MVM_OK;
 }
 int maxpool2(const float* in, float* out, int B, int H, int W, int C, cudaStream_t s) {
-  sp_maxpool2_kernel<<<148 * 8, 256, 0, s>>>(in, out, B, H, W, C);
+  sp_maxpool2_kernel<<<mvm_dev_info().n_sm * 8, 256, 0, s>>>(in, out, B, H, W, C);
   MVM_CHECK_LAUNCH();
   return MVM_OK;
 }
 int maxfilter(const float* in, float* tmp, float* out, int B, int H, int W, int r, cudaStream_t s) {
-  sp_maxrow_kernel<<<148 * 4, 256, 0, s>>>(in, tmp, B, H, W, r);
+  sp_maxrow_kernel<<<mvm_dev_info().n_sm * 4, 256, 0, s>>>(in, tmp, B, H, W, r);
   MVM_CHECK_LAUNCH();
-  sp_maxcol_kernel<<<148 * 4, 256, 0, s>>>(tmp, out, B, H, W, r);
+  sp_maxcol_kernel<<<mvm_dev_info().n_sm * 4, 256, 0, s>>>(tmp, out, B, H, W, r);
   MVM_CHECK_LAUNCH();
   return MVM_OK;
 }
@@ -322,7 +322,7 @@ int mvm_superpoint_dense(const mvm_superpoint_weights* wt, const float* image, i
   // simple_nms (:47-63)
   {
     const long long n = (long long)px;
-    const int blocks = 148 * 4;
+    const int blocks = mvm_dev_info().n_sm * 4;
     SP_TRY(maxfilter(P0, P4, P1, batch, height, width, nms_radius, s));          // P1 = max_pool(scores)
     sp_nms_init_kernel<<<blocks, 256, 0, s>>>(P0, P1, P2, n);                    // P2 = max_mask
     MVM_CHECK_LAUNCH();

@@ -77,7 +77,7 @@ int mvm_match_loss_backward(const int64_t* gt_indices, const float* gt_weights, 
   MVM_REQUIRE(gt_indices && gt_weights && grad_loss && grad_log_p && bs >= 1 && ft >= 2);
   MvmProfScope prof__(MVM_TAG_MISC, s);
   cudaMemsetAsync(grad_log_p, 0, (size_t)bs * ft * ft * sizeof(float), s);
-  match_loss_bwd_kernel<<<148 * 2, 256, 0, s>>>((const long long*)gt_indices, gt_weights, grad_loss, grad_log_p, bs, ft);
+  match_loss_bwd_kernel<<<mvm_dev_info().n_sm * 2, 256, 0, s>>>((const long long*)gt_indices, gt_weights, grad_loss, grad_log_p, bs, ft);
   MVM_CHECK_LAUNCH();
   return MVM_OK;
 }

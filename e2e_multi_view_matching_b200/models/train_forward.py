@@ -6,7 +6,7 @@ running-statistics updates (:8-22), combined cross attention over the other view
 `loss.backward()` computes for the reference when it trains on the match loss (train.py stage 1, helpers.py:228-260).
 
 The eval forward runs as one fused C call on packed weights with the BatchNorms folded into the convolutions; batch
-statistics cannot be folded, so the train branch sequences the stage kernels from Python: tcgen05 GEMMs (fp16x3 forward,
+statistics cannot be folded, so the train branch sequences the stage kernels from Python: tensor-core GEMMs (fp16x3 forward,
 3xTF32 backward -- gradients need the fp32 exponent range), the fp16x3 attention forward, `mvm_attention_backward`,
 `mvm_batchnorm_train[_backward]`, `mvm_sinkhorn_train_{forward,backward}` (exact gradient of the unrolled iterations).
 The whole matcher is ONE autograd.Function (`MatcherTrainFn`): its inputs are the module's parameters, its outputs the
@@ -31,7 +31,7 @@ def _head_perm(device):
 
 
 def _lin(x, w, b, relu=False, a2=None, residual=None, alpha=1.0):
-    """Conv1d(k=1) on point-major rows: tcgen05 fp16x3 when the shape allows, fp32 CUDA cores otherwise."""
+    """Conv1d(k=1) on point-major rows: tensor-core fp16x3 when the shape allows, fp32 CUDA cores otherwise."""
     w = w.detach().float().contiguous()
     b = None if b is None else b.detach().float().contiguous()
     K = x.shape[1] + (a2.shape[1] if a2 is not None else 0)

@@ -14,7 +14,7 @@ def rn_tf32(x):
 
 def linear(a, w, bias=None, a2=None, residual=None, relu=False, alpha=1.0, tc_passes=0, presplit=False):
     """act(alpha * [a|a2] @ w.T + bias) + residual on point-major activations (Conv1d k=1).
-    tc_passes: 0 = fp32 CUDA cores, 3 = tcgen05 3xTF32, 1 = tcgen05 single-pass TF32.
+    tc_passes: 0 = fp32 CUDA cores, 3 = 3xTF32 on the tensor cores, 1 = single-pass TF32.
     presplit (with tc_passes=3): hand W over as its tf32 hi/lo planes, like the packed matcher weights do --
     this is the production path (persistent kernel)."""
     lib = _lib.lib()
@@ -187,7 +187,7 @@ def transpose_split(x, raw=False, planes=True, out=None):
 
 
 def linear_presplit(a, w_hi, w_lo, residual=None, alpha=1.0):
-    """alpha * a [M, K] @ w^T + residual with w [N, K] given as its tf32 planes: the 3xTF32 tcgen05 GEMM (fp32 range --
+    """alpha * a [M, K] @ w^T + residual with w [N, K] given as its tf32 planes: the 3xTF32 tensor-core GEMM (fp32 range --
     the half-precision planes of the inference path would flush small gradients)."""
     lib = _lib.lib()
     M, K = a.shape
@@ -242,7 +242,10 @@ def gemm_dw(dy, x, x2=None, alpha=1.0):
         # few output tiles, a very long contraction: cut K = rows into slices for different CTAs (split-K)
         tiles = (n_out // 128) * (k_in // 128) if n_out % 128 == 0 else 0
         kb = rows // 32
-        ks = max([s_ for s_ in range(1, 65) if kb % s_ == 0 and kb // s_ >= 8 and tiles * s_ <= 148] or [1]) if tiles else 1
+        # (the CPU stand-ins of the tests take the split of the GPU they run beside; 132 = H100 SXM without one)
+        n_sm = torch.cuda.get_device_properties(dev if dev.type == 'cuda' else torch.cuda.current_device()).multi_processor_count \
+            if torch.cuda.is_available() else 132
+        ks = max([s_ for s_ in range(1, 65) if kb % s_ == 0 and kb // s_ >= 8 and tiles * s_ <= n_sm] or [1]) if tiles else 1
         if ks >= 2:
             return linear_presplit_splitk(dyt, hi, lo, ks, alpha=alpha)
         return linear_presplit(dyt, hi, lo, alpha=alpha)
@@ -315,7 +318,7 @@ def attention_backward(qkv, out, dout, batch, n_views, counts, is_cross):
 def pair_scores(md, pairs, N, alpha=1.0 / 16.0):
     """md [B, T, n_pad, 256] matching descriptors, pairs [(slot a, slot b)] -> score buffers [P * B, N + 1, N + 1] whose
     inner blocks hold md_a md_b^T * alpha (pair-major; the dustbin row / column are left unset): one launch of the
-    persistent tcgen05 GEMM's score mode (mvm_pair_scores)."""
+    tensor-core GEMM's score mode (mvm_pair_scores)."""
     lib = _lib.lib()
     B, T, n_pad, _ = md.shape
     P = len(pairs)

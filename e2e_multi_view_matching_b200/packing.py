@@ -1,4 +1,4 @@
-"""Repack a reference state dict for the B200 kernels.
+"""Repack a reference state dict for the H100 kernels.
 
 * eval-mode BatchNorm1d folded into the preceding 1x1 conv:
     W' = W * g / sqrt(var + eps),  b' = (b - mean) * g / sqrt(var + eps) + beta

@@ -95,7 +95,7 @@ def initialize_bundle_adjust(n_images, data, result, file_path, conf_thresh=0., 
     if rel_pose_method != "w8pt_ba":
         if rel_pose_method in ("ransac", "ransac_ba"):
             raise NotImplementedError("rel_pose_method '{}' is an OpenCV CPU baseline of the reference; only 'w8pt_ba' "
-                                      "runs on the B200 path".format(rel_pose_method))
+                                      "runs on the GPU path".format(rel_pose_method))
         logging.error("Relative pose estimation method {} is not defined".format(rel_pose_method))
     pair_wise_data = dict()
     for id0, id1 in _all_pairs(n_images):

@@ -1,4 +1,4 @@
-/* mvm_b200.h -- C ABI of libmvm_b200.so, the B200 (sm_100a) drop-in for the hot path of
+/* mvm_b200.h -- C ABI of libmvm_b200.so, the H100 (sm_90a) drop-in for the hot path of
  * barbararoessle/e2e_multi_view_matching.
  *
  * The reference has no FFI layer: the path sits behind Python callables.  Each entry point
@@ -118,13 +118,13 @@ int mvm_matcher_forward(const mvm_matcher_weights* w, int batch, int n_views, in
  * score kernel, 256-wide persistent GEMM, automatic Sinkhorn kernel), which mvm_set_math_mode / the mvm_debug_*
  * hooks below change for callers of the plain mvm_matcher_forward. */
 typedef struct mvm_matcher_options {
-  int math_mode;        /* 3 = tcgen05 3xTF32 (fp32-faithful), 1 = tcgen05 single-pass TF32, 0 = fp32 CUDA cores */
+  int math_mode;        /* 3 = 3xTF32 on the tensor cores (fp32-faithful), 1 = single-pass TF32, 0 = fp32 CUDA cores */
   int score_kernel;     /* 1 = score matrices on the tensor cores (math mode 3), 0 = fp32 CUDA cores */
   int gemm_tile;        /* 128 | 256: tile width of the one-tile-per-CTA GEMM (when gemm_kernel == 0) */
   int gemm_kernel;      /* 1 = persistent 3xTF32 GEMM, 0 = one tile per CTA */
   int sinkhorn_variant; /* 0 = automatic (see mvm_log_optimal_transport_ex) */
-  int attention_split;  /* math mode 3: operand planes of attention, 0 = tf32 hi/lo (3 x kind::tf32), 1 = fp16 hi/lo
-                         * (3 x kind::f16: same 22-bit operands, half the tensor-pipe time) */
+  int attention_split;  /* math mode 3: operand planes of attention, 0 = tf32 hi/lo (3 x tf32 wgmma), 1 = fp16 hi/lo
+                         * (3 x f16 wgmma: same 22-bit operands, half the tensor-pipe time) */
   int gemm_split;       /* the same choice for the 1x1-conv GEMMs (1 needs mvm_matcher_weights.w16_*) */
 } mvm_matcher_options;
 void mvm_matcher_options_default(mvm_matcher_options* opt);
@@ -143,7 +143,7 @@ int mvm_linear(const float* A, int lda, const float* A2, int lda2, int K1, const
                int ldw, const float* bias, const float* R, int ldr, float* C, int ldc, int M,
                int N, int K, float alpha, int relu, void* stream);
 
-/* Same contract on the tensor cores (tcgen05.mma kind::tf32, TMA-fed, TMEM accumulator).
+/* Same contract on the tensor cores (tf32 wgmma, TMA-fed, accumulators in registers).
  * n_pass = 3: fp32-faithful 3xTF32 (operands split hi/lo on chip); n_pass = 1: single-pass TF32.
  * Needs N % 128 == 0, K % 32 == 0, K1 % 32 == 0, 16-byte aligned rows. */
 int mvm_linear_tc(const float* A, int lda, const float* A2, int lda2, int K1, const float* W,
@@ -151,8 +151,8 @@ int mvm_linear_tc(const float* A, int lda, const float* A2, int lda2, int K1, co
                   int N, int K, float alpha, int relu, int n_pass, void* stream);
 
 /* The production 3xTF32 path: W given as its two tf32 planes W_hi = rn_tf32(W), W_lo = rn_tf32(W - W_hi)
- * (what packing.py stores next to the raw weights).  Persistent kernel: A split on chip into tensor memory,
- * two TMEM accumulators, TMA-store epilogue.  Same shape requirements as mvm_linear_tc. */
+ * (what packing.py stores next to the raw weights).  Persistent schedule, A split on chip in
+ * registers.  Same shape requirements as mvm_linear_tc. */
 int mvm_linear_tc_presplit(const float* A, int lda, const float* A2, int lda2, int K1, const float* W_hi,
                            const float* W_lo, int ldw, const float* bias, const float* R, int ldr, float* C,
                            int ldc, int M, int N, int K, float alpha, int relu, void* stream);
@@ -163,14 +163,14 @@ int mvm_linear_tc_presplit(const float* A, int lda, const float* A2, int lda2, i
 int mvm_linear_tc_presplit_splitk(const float* A, int lda, const float* W_hi, const float* W_lo, int ldw, float* C, int ldc,
                                   int M, int N, int K, float alpha, int ksplit, float* ws, void* stream);
 
-/* fp16x3 on the persistent kernel: W16_hi / W16_lo = fp16 planes of wscale * W (hi = fp16(wscale W), lo = fp16(wscale W - hi));
+/* fp16x3 on the persistent schedule: W16_hi / W16_lo = fp16 planes of wscale * W (hi = fp16(wscale W), lo = fp16(wscale W - hi));
  * K and K1 multiples of 64, N of 128. */
 int mvm_linear_tc_h16(const float* A, int lda, const float* A2, int lda2, int K1, const void* W16_hi, const void* W16_lo,
                       float wscale, int ldw, const float* bias, const float* R, int ldr, float* C, int ldc, int M, int N, int K,
                       float alpha, int relu, void* stream);
 
 /* Math mode of the matcher's GEMMs/attention inside mvm_matcher_forward: 0 = fp32 CUDA cores,
- * 3 = tcgen05 3xTF32 (fp32-faithful), 1 = tcgen05 single-pass TF32 (torch 1.10's Ampere default). */
+ * 3 = 3xTF32 on the tensor cores (fp32-faithful), 1 = single-pass TF32 (torch 1.10's Ampere default). */
 int mvm_set_math_mode(int mode);
 int mvm_get_math_mode(void);
 
@@ -181,7 +181,7 @@ int mvm_get_math_mode(void);
 int mvm_attention(const float* qkv, float* out, int batch, int n_views, int n_pad,
                   const int* counts, int is_cross, void* stream);
 
-/* The same attention on the tensor cores (tcgen05/TMEM/TMA flash kernel).  vt [n_views_total, 256,
+/* The same attention on the tensor cores (wgmma/TMA flash kernel).  vt [n_views_total, 256,
  * n_pad] holds V^T per head (written by the QKV GEMM epilogue); the v third of qkv is not read.
  * n_pass == 3 (3xTF32): the k third of qkv and vt must hold rn_tf32 values and klo [rows,256] / vtlo
  * their tf32-rounded remainders (the QKV GEMM epilogue writes all four); NULL for n_pass == 1. */
@@ -190,7 +190,7 @@ int mvm_attention_tc(const float* qkv, const float* vt, float* out, int batch, i
                      void* stream);
 
 /* fp32-faithful attention with HALF-PRECISION operand planes (fp16x3: hi = fp16(x), lo = fp16(x - hi); three
- * kind::f16 MMAs per product, half the tensor-pipe time of the tf32 variant at the same 22-bit operand precision).
+ * f16 MMAs per product, half the tensor-pipe time of the tf32 variant at the same 22-bit operand precision).
  * kh, kl, vh, vl [n_views_total * n_pad, 256] are fp16 buffers, point-major like K and V themselves (the QKV GEMM
  * epilogue writes them inside mvm_matcher_forward; V is read as an MN-major tensor-core operand, no transposed copy);
  * the q third of qkv is read as fp32. */
@@ -397,7 +397,7 @@ int mvm_attention_backward(const float* qkv, const float* out, const float* dout
  * 0 = fp32 CUDA cores (cross-check) */
 int mvm_debug_set_attention_backward_variant(int variant);
 
-/* Every (pair, tuple) score matrix of a call in one launch of the persistent tcgen05 GEMM (3xTF32):
+/* Every (pair, tuple) score matrix of a call in one launch of the tensor-core GEMM (3xTF32):
  * scores[p][bi] inner [m_p, n_p] block = mdesc[view a_p of tuple bi] . mdesc[view b_p of tuple bi]^T * alpha, written
  * into buffers laid out [batch, m_p + 1, n_p + 1] (multi_view_matcher.py:278-280; the dustbin row / column are not
  * touched).  mdesc: [batch * n_views * n_pad, 256] point-major; hi / lo: scratch of the same size; pa / pb / m / n and
@@ -452,7 +452,7 @@ void mvm_debug_set_attention_timing(long long* buf);
 void mvm_debug_set_sinkhorn_timing(long long* buf);
 void mvm_debug_set_mvba_timing(long long* buf);
 
-/* Library/build info: returns "mvm_b200 <version> sm_100a". */
+/* Library/build info: returns "mvm_b200 <version> sm_90a". */
 const char* mvm_version(void);
 
 #ifdef __cplusplus

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
 
 
 @pytest.fixture(scope='session')
@@ -19,7 +19,7 @@ def golden_dir():
 
 @pytest.fixture(autouse=True)
 def _default_math_mode(request):
-    """Every GPU test starts from the library default (tcgen05 3xTF32) regardless of what ran before."""
+    """Every GPU test starts from the library default (3xTF32 on the tensor cores) regardless of what ran before."""
     if request.node.get_closest_marker('gpu') is not None:
         import e2e_multi_view_matching_b200 as pkg
         pkg.set_math_mode(3)

@@ -25,7 +25,7 @@ def test_library_exports_declared_symbols():
     for n in names:
         assert hasattr(lib, n), 'missing symbol %s' % n
     lib.mvm_version.restype = ctypes.c_char_p
-    assert b'sm_100a' in lib.mvm_version()
+    assert b'sm_90a' in lib.mvm_version()
 
 
 def test_struct_layout_matches_header():

@@ -24,8 +24,8 @@ def test_pose_auc_engine_equals_oracle(config):
     assert r['oracle'][2] > 30.0, 'the synthetic setup should give a meaningful AUC'
     # Two-view path: equal to 0.1 pt (measured 3e-4 pt).  Multi-view path: the global LM bundle adjustment of a tuple whose
     # problem is poorly conditioned (free scale gauge) stops after a different number of iterations in the two
-    # implementations (same cost to 0.5 %, poses up to ~2 deg apart on 5 of 32 tuples; tools/auc_diag.py,
-    # profiles/r02_auc_diag.txt) -- unpinned against Ceres' exact iterates on both sides (DESIGN.md §5): 0.5 pt, and the
+    # implementations (same cost to 0.5 %, poses up to ~2 deg apart on 5 of 32 tuples; tools/auc_diag.py)
+    # -- unpinned against Ceres' exact iterates on both sides (DESIGN.md §5): 0.5 pt, and the
     # median pair must agree to 0.01 deg.
     assert r['max_abs_diff_pt'] <= (0.1 if config == 'cfg2' else 0.5), r
     assert r['median_abs_pose_error_diff_deg'] < 1e-2, r

@@ -1,4 +1,4 @@
-"""fp16x3 attention (attention_h3.cu): hi = fp16(x), lo = fp16(x - hi) operand planes, three kind::f16 MMAs per product.
+"""fp16x3 attention (attention_h3.cu): hi = fp16(x), lo = fp16(x - hi) operand planes, three f16 MMAs per product.
 Stage parity against the fp32 CUDA-core attention, and the whole matcher with this variant against the reference
 goldens at the same tolerances as the tf32x3 default."""
 import json

@@ -59,7 +59,7 @@ def test_full_size_matcher_vs_reference(name):
             # ---- whole-matrix checksums: mean signed error and mean square ----
             chk = z['chk_' + sk]
             numel = Zc[0].size
-            # (the split-operand arithmetic carries a systematic +1e-5 .. +1e-4 bias, profiles/r02_score_ab.txt: this is a
+            # (the split-operand arithmetic carries a systematic +1e-5 .. +1e-4 bias (tools/score_ab.py): this is a
             # gross-error check -- a dropped row or column shifts the mean by far more)
             assert np.abs(Zc.sum((1, 2)) - chk[:, 0]).max() / numel < 2e-4, sk
             assert np.abs((Zc * Zc).sum((1, 2)) - chk[:, 1]).max() / np.abs(chk[:, 1]).max() < 1e-4, sk

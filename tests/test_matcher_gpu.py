@@ -27,7 +27,7 @@ def run_ours(meta, sd, data):
 @pytest.mark.parametrize('mode', [3, 0])
 @pytest.mark.parametrize('name', MATCHER_CASES)
 def test_matcher_matches_reference_golden(name, mode):
-    """mode 3 = the default tensor-core path (tcgen05, 3xTF32: fp32-faithful to ~1e-5 relative on the
+    """mode 3 = the default tensor-core path (3xTF32: fp32-faithful to ~1e-5 relative on the
     coupling matrices), mode 0 = the fp32 CUDA-core cross-check path (tighter)."""
     import e2e_multi_view_matching_b200 as pkg
     meta, ref = load_case(name)

@@ -1,4 +1,4 @@
-"""GPU: tcgen05 tensor-core kernels against fp64 math and the fp32 CUDA-core kernels."""
+"""GPU: tensor-core (wgmma) kernels against fp64 math and the fp32 CUDA-core kernels."""
 import numpy as np
 import pytest
 import torch
@@ -33,7 +33,7 @@ def test_gemm_tc_vs_fp64(shape, passes):
 @pytest.mark.parametrize('name', ['pair_small_ragged', 'pair_18l_128_sharp', 'mv5_28l_96_sharp', 'mv4_ragged_sharp'])
 @pytest.mark.parametrize('mode', [3, 1])
 def test_matcher_tensor_core_modes(name, mode):
-    """Whole matcher with the GEMMs (and attention, once enabled) on tcgen05: 3xTF32 keeps the fp32
+    """Whole matcher with the GEMMs (and attention) on the tensor cores: 3xTF32 keeps the fp32
     parity contract; single-pass TF32 (torch 1.10's Ampere default) is compared at TF32 accuracy."""
     import e2e_multi_view_matching_b200 as pkg
     from tests.util import load_case, case_inputs, compare_matcher_outputs, score_tol_for

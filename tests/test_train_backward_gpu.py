@@ -175,7 +175,7 @@ def test_backward_system_vs_standins_on_the_gpu_forward_state(name, monkeypatch)
     """The whole backward (every kernel in sequence, 100+ launches) against the float64 stand-ins run on the SAME saved
     forward state (the GPU's activations, BatchNorm statistics and ReLU masks): isolates the backward kernels from the
     rounding of the forward -- a pre-ReLU activation within ~1e-5 of zero flips its mask between two correct forwards,
-    which moves the gradient by far more than rounding does (profiles/r02_train_kink.txt)."""
+    which moves the gradient by far more than rounding does (tools/train_kink_experiment.py)."""
     import copy
     from e2e_multi_view_matching_b200 import ops, _lib
     from e2e_multi_view_matching_b200.models import train_forward as TF
@@ -224,7 +224,7 @@ def test_train_step_vs_reference_golden(name):
     reference's own fp32 deviation.  The gradients are bounded by what ONE flipped ReLU mask does (the measured error /
     reference-deviation ratios are printed: median 2-11, i.e. most parameters sit within a few times the reference's own
     fp32-vs-fp64 deviation when no mask flips upstream of them) (an activation within ~1e-5 of zero has a different sign in two correctly rounded forwards: measured
-    on the float64 stand-ins with a 1e-6 forward perturbation, profiles/r02_train_kink.txt: up to 7e-3 of the gradient's
+    on the float64 stand-ins with a 1e-6 forward perturbation (tools/train_kink_experiment.py): up to 7e-3 of the gradient's
     scale) -- 2e-2 of the parameter's gradient scale.  The backward itself is pinned tighter by the test above."""
     from tests.test_train_host_logic import check_gradients
     z, case, model, data = _golden_case(name)

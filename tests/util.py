@@ -32,7 +32,7 @@ def score_tol_for(name):
     """(abs, rel) tolerance on the log-couplings of a golden case in the default fp32-faithful tensor-core mode.  The
     reference's own fp32 run sits `noise` away from its double-precision run (matcher_report.json, measured by the
     generator).  The split-operand arithmetic (22-bit operands, lo.lo term dropped) is measured at up to 3.6x that noise
-    in absolute terms on top of a 3e-5 relative term (tools/score_ab.py, profiles/r02_score_ab.txt; the fp32 CUDA-core
+    in absolute terms on top of a 3e-5 relative term (tools/score_ab.py; the fp32 CUDA-core
     mode sits AT the noise): 4x noise, never below 3e-4."""
     noise = json.load(open(os.path.join(GOLDEN, 'matcher_report.json')))[name]['max_abs_ref32_vs_ref64']
     return (max(3e-4, 4.0 * noise), 3e-5)
