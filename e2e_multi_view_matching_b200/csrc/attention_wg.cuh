@@ -3,10 +3,10 @@
 // concatenation of the other views (multi_view_matcher.py:76-78,92-95).  prob[B,4,N,M] is never materialised.
 //
 // One CTA = 128 queries of one (view, head); keys / values stream through in tiles of 64.  288 threads:
-//   warps 0-3, 4-7   two consumer warpgroups, queries [0,64) and [64,128) of the block: Q fragments in registers
-//                    (split into hi / lo per key tile), S = Q K^T with wgmma (B = K tile in shared memory), online softmax on
-//                    the accumulator registers (a row lives in the four threads of a quad), P re-packed in registers
-//                    as the A operand of O += P V (B = V tile in shared memory); O stays in registers until the end
+//   warps 0-3, 4-7   two consumer warpgroups, queries [0,64) and [64,128) of the block: S = Q K^T with wgmma (B = K
+//                    tile in shared memory), online softmax on the accumulator registers (a row lives in the four
+//                    threads of a quad), P re-packed in registers as the A operand of O += P V (B = V tile in shared
+//                    memory); O stays in registers until the end
 //   warp 8           TMA producer: the K and V planes of every key tile into ST-deep rings
 // Operand arithmetic (MODE):
 //   1   single-pass TF32: K from the fused QKV projection [rows, 768], V^T [view * 256 + h * 64 + d, key] written by the
@@ -15,7 +15,15 @@
 //       written by the QKV GEMM epilogue, Q and P are split in registers
 //   16  fp16x3: the same three products on half-precision hi / lo planes (hi = fp16(x), lo = fp16(x - hi): 22 bits like
 //       the tf32 pair) at K = 16 per instruction; K and V planes [rows, 256] come from the QKV GEMM epilogue and V is
-//       read key-major as an MN-major B operand (no transposed copy)
+//       read key-major as an MN-major B operand (no transposed copy); Q is split once into hi / lo planes in shared
+//       memory (A operand of S = Q K^T from shared memory)
+// Schedule (MODE 16): inside a warpgroup, S(j+1) = Q K(j+1)^T and O += P(j) V(j) are issued back to back and the
+// softmax of tile j+1 runs while P(j) V(j) is on the tensor cores; across the two warpgroups, named barriers make them
+// take turns issuing (FlashAttention-3 §3.1 ping-pong), so one warpgroup's MMAs cover the other's softmax.  The tf32
+// modes run each tile's S, softmax and P V in order: in MODE 3 the Q split of S(j+1) next to P(j) in flight does not
+// fit the registers; MODE 1 showed no gain beyond run-to-run noise from the ping-pong alone and has not been measured
+// with the overlap inside a warpgroup.
+// Every schedule does the same operations on every output element in the same order: the results are identical.
 #pragma once
 #include <cuda_fp16.h>
 #include "common.cuh"
@@ -27,16 +35,22 @@ namespace attn_wg {
 constexpr int BQ = 128, BKV = 64, HD = 64;
 constexpr int NTHREADS = 288;
 constexpr int PRODUCER_WARP = 8;
+// named barriers (0 is __syncthreads): warpgroup w may issue its MMAs once PP_BAR + w completes; Q_BAR + w orders a
+// warpgroup's shared-memory Q stores before its first wgmma
+constexpr int PP_BAR = 1, Q_BAR = 3;
 
 template <int MODE>
 struct Cfg {
   static constexpr bool F16 = MODE == 16;
+  static constexpr bool PIPE = F16;                           // pipelined + ping-pong schedule
   static constexpr int PL = MODE == 1 ? 1 : 2;                // operand planes per tile (hi [, lo])
   static constexpr int PLANE = F16 ? 8192 : 16384;            // [64 x 64]: one fp16 box or two [64 x 32] fp32 boxes
   static constexpr int TILE = PL * PLANE;
   static constexpr int ST = MODE == 3 ? 3 : 4;                // ring depth of K and of V
   static constexpr int OFF_V = ST * TILE;
-  static constexpr int OFF_BAR = 2 * ST * TILE;
+  static constexpr int OFF_Q = 2 * ST * TILE;                 // MODE 16: Q hi, Q lo [128 x 64] fp16, 128B-swizzled
+  static constexpr int QPLANE = BQ * 128;
+  static constexpr int OFF_BAR = OFF_Q + (F16 ? 2 * QPLANE : 0);
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 };
 
@@ -64,6 +78,20 @@ __device__ __forceinline__ void split_pack(float x0, float x1, uint32_t& hi, uin
   hi = *reinterpret_cast<const uint32_t*>(&h);
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
+__device__ __forceinline__ void named_bar_sync(int id, int n) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int n) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+// A-operand registers of an issued wgmma stay live (and unchanged) until this point, after the wait that retires it
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (*a)[4]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) asm volatile("" : "+r"(a[i][e])::"memory");
+}
 
 template <int MODE>
 __global__ void __launch_bounds__(NTHREADS, 1)
@@ -71,7 +99,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
                     const __grid_constant__ CUtensorMap tmKlo, const __grid_constant__ CUtensorMap tmVlo,
                     const __grid_constant__ Args g) {
   using C_ = Cfg<MODE>;
-  constexpr bool F16 = C_::F16;
+  constexpr bool F16 = C_::F16, PIPE = C_::PIPE;
   constexpr int ST = C_::ST, PLANE = C_::PLANE, TILE = C_::TILE;
   constexpr int KS = F16 ? 4 : 8;                             // K steps over d (S) and over keys (P V)
   extern __shared__ uint8_t smem_raw[];
@@ -152,8 +180,9 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   const int gr = lane >> 2, tq = lane & 3;
   const int lrow = wg * 64 + wq * 16 + gr;                      // query rows of this thread: lrow, lrow + 8
   // Q fragments, raw fp32 (rows past the view are read but never written back; rows past the buffer read as zero).
-  // They are split into the hi / lo wgmma operands inside the key-tile loop: when the operand registers were only
-  // defined before the loop, ptxas (CUDA 12.9) reused them inside the loop body and later tiles read stale Q_lo.
+  // MODE 16 splits them once into the swizzled hi / lo planes.  The tf32 modes keep them in registers and split them
+  // inside the key-tile loop: when the operand registers were only defined before the loop, ptxas (CUDA 12.9) reused
+  // them inside the loop body and later tiles read stale Q_lo.
   float2 qraw[KS][4];
   {
     const long long total = (long long)gridDim.z * g.n_pad;
@@ -179,6 +208,24 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
       }
     }
   }
+  if constexpr (F16) {
+    // element pair (row r, cols 16 kk + 2 tq + 8 (e >> 1)) -> 16-byte chunk 2 kk + (e >> 1) of the 128-byte row r, XOR
+    // r % 8 (= gr): the layout TMA's 128B swizzle gives the K planes
+    uint8_t* sq = smem + C_::OFF_Q + lrow * 128 + 4 * tq;
+#pragma unroll
+    for (int kk = 0; kk < KS; ++kk) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        uint32_t hi, lo;
+        split_pack(qraw[kk][e].x, qraw[kk][e].y, hi, lo);
+        const int off = (e & 1) * 1024 + (((2 * kk + (e >> 1)) ^ gr) << 4);
+        *reinterpret_cast<uint32_t*>(sq + off) = hi;
+        *reinterpret_cast<uint32_t*>(sq + C_::QPLANE + off) = lo;
+      }
+    }
+    tc::fence_proxy_async();                                    // generic-proxy stores -> wgmma reads
+    named_bar_sync(Q_BAR + wg, 128);
+  }
 
   // online softmax in log2 units (scores * log2(e) / sqrt(d)); row hh of this thread = lrow + 8 hh.  The reference m of
   // a row is only raised (and O, l rescaled) when the row maximum outgrows it by more than 2^8, and P is taken relative
@@ -190,6 +237,187 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   const float scale_l2e = 0.125f * 1.4426950408889634f;
   const int srcA = (lane & ~3) | (tq >> 1), srcB = srcA + 2;   // tf32 P fragments: owners of keys tq and tq + 4
+  float sc[32], fo[2];                                          // fo: rescale of O by the last softmax (1: none)
+  uint32_t qhi[KS][4], qlo[KS][4];                              // tf32 modes: the Q operand of S
+  uint32_t phi[KS][4], plo[KS][4];                              // P of a softmax: the A operand of its P V
+
+  auto prep_s = [&] {
+    if constexpr (!F16) {
+#pragma unroll
+      for (int kk = 0; kk < KS; ++kk) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          float x = qraw[kk][e].x;
+          asm volatile("" : "+f"(x));                           // keeps the split inside the loop (no hoisting)
+          const float hi = MODE == 3 ? tf32_hi(x) : x;
+          qhi[kk][e] = __float_as_uint(hi);
+          qlo[kk][e] = __float_as_uint(MODE == 3 ? tf32_hi(x - hi) : 0.f);
+        }
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) sc[i] = 0.f;
+    tc::fence_acc<64>(sc);                                      // zeroed before the wgmma fence
+  };
+  // ---- S = Q K^T on the K tile of ring stage st (issue only)
+  auto issue_s = [&](int st, uint32_t ph) {
+    tc::mbar_wait(k_full + st, ph);
+    const uint32_t kb = tc::smem_u32(smem + st * TILE);
+    tc::wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < KS; ++kk) {
+      if (F16) {
+        const uint32_t qb = tc::smem_u32(smem + C_::OFF_Q + wg * 64 * 128) + kk * 32;
+        const uint64_t dq = tc::make_sw128_desc(qb), dk = tc::make_sw128_desc(kb + kk * 32);
+        tc::wgmma_f16_ss<64>(sc, dq, dk);
+        tc::wgmma_f16_ss<64>(sc, dq, tc::make_sw128_desc(kb + PLANE + kk * 32));
+        tc::wgmma_f16_ss<64>(sc, tc::make_sw128_desc(qb + C_::QPLANE), dk);
+      } else {
+        const uint32_t off = (kk >> 2) * 8192 + (kk & 3) * 32;
+        const uint64_t dk = tc::make_sw128_desc(kb + off);
+        tc::wgmma_tf32_rs<64>(sc, qhi[kk], dk);
+        if (MODE == 3) {
+          tc::wgmma_tf32_rs<64>(sc, qhi[kk], tc::make_sw128_desc(kb + PLANE + off));
+          tc::wgmma_tf32_rs<64>(sc, qlo[kk], dk);
+        }
+      }
+    }
+    tc::wgmma_commit();
+  };
+  // after the wait that retired the S of ring stage st
+  auto retire_s = [&](int st) {
+    tc::fence_acc<64>(sc);
+    if constexpr (!F16) { fence_regs<KS>(qhi); fence_regs<KS>(qlo); }
+    tc::mbar_arrive(k_empty + st);
+  };
+  // ---- O += P V on the V tile of ring stage st (issue only)
+  auto issue_pv = [&](int st, uint32_t ph) {
+    tc::mbar_wait(v_full + st, ph);
+    const uint32_t vb = tc::smem_u32(smem + C_::OFF_V + st * TILE);
+    tc::wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < KS; ++kk) {
+      if (F16) {
+        const uint64_t dv = tc::make_sw128_desc(vb + kk * 2048);      // 16 keys x 128 B, V key-major (MN-major B)
+        tc::wgmma_f16_rs<64, 1>(o, phi[kk], dv);
+        tc::wgmma_f16_rs<64, 1>(o, phi[kk], tc::make_sw128_desc(vb + PLANE + kk * 2048));
+        tc::wgmma_f16_rs<64, 1>(o, plo[kk], dv);
+      } else {
+        const uint32_t off = (kk >> 2) * 8192 + (kk & 3) * 32;
+        const uint64_t dv = tc::make_sw128_desc(vb + off);
+        tc::wgmma_tf32_rs<64>(o, phi[kk], dv);
+        if (MODE == 3) {
+          tc::wgmma_tf32_rs<64>(o, phi[kk], tc::make_sw128_desc(vb + PLANE + off));
+          tc::wgmma_tf32_rs<64>(o, plo[kk], dv);
+        }
+      }
+    }
+    tc::wgmma_commit();
+  };
+  // after the wait that retired the P V of ring stage st
+  auto retire_pv = [&](int st) {
+    tc::fence_acc<64>(o);
+    fence_regs<KS>(phi);
+    fence_regs<KS>(plo);
+    tc::mbar_arrive(v_empty + st);
+  };
+  // ---- online softmax of S in place (a row is spread over the four threads of a quad); sets fo, leaves O alone
+  auto softmax = [&](int nvalid) {
+    if (nvalid < BKV) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int key = 8 * i + 2 * tq;
+        if (key >= nvalid) { sc[4 * i] = -INFINITY; sc[4 * i + 2] = -INFINITY; }
+        if (key + 1 >= nvalid) { sc[4 * i + 1] = -INFINITY; sc[4 * i + 3] = -INFINITY; }
+      }
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float mx = sc[2 * hh];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * hh], sc[4 * i + 2 * hh + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      mx *= scale_l2e;
+      fo[hh] = 1.f;
+      if (mx > m_run[hh] + 8.f) {                               // the same decision in the four threads of the quad
+        fo[hh] = ex2_ftz(m_run[hh] - mx);                       // < 2^-8
+        m_run[hh] = mx;
+        l_run[hh] *= fo[hh];
+      }
+      const float nm = 7.f - m_run[hh];
+      float rs = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float p0 = ex2_ftz(fmaf(sc[4 * i + 2 * hh], scale_l2e, nm));
+        const float p1 = ex2_ftz(fmaf(sc[4 * i + 2 * hh + 1], scale_l2e, nm));
+        sc[4 * i + 2 * hh] = p0;
+        sc[4 * i + 2 * hh + 1] = p1;
+        rs += p0 + p1;
+      }
+      l_run[hh] += rs;
+    }
+  };
+  auto rescale_o = [&] {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      if (fo[hh] != 1.f) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          o[4 * i + 2 * hh] *= fo[hh];
+          o[4 * i + 2 * hh + 1] *= fo[hh];
+        }
+      }
+    }
+  };
+  // ---- P as the register A operand of O += P V
+  auto split_p = [&] {
+#pragma unroll
+    for (int kk = 0; kk < KS; ++kk) {
+      if (F16) {
+        // the accumulator layout of keys [16 kk, 16 kk + 16) is the k16 A fragment layout
+#pragma unroll
+        for (int e = 0; e < 4; ++e) split_pack(sc[8 * kk + 2 * e], sc[8 * kk + 2 * e + 1], phi[kk][e], plo[kk][e]);
+      } else {
+        // k8 A fragment: keys tq and tq + 4 of the step, held by quad lanes tq / 2 and 2 + tq / 2
+        float a[4];
+        const bool odd = tq & 1;
+        const float x0 = __shfl_sync(0xffffffffu, sc[4 * kk], srcA), x1 = __shfl_sync(0xffffffffu, sc[4 * kk + 1], srcA);
+        const float y0 = __shfl_sync(0xffffffffu, sc[4 * kk + 2], srcA), y1 = __shfl_sync(0xffffffffu, sc[4 * kk + 3], srcA);
+        const float z0 = __shfl_sync(0xffffffffu, sc[4 * kk], srcB), z1 = __shfl_sync(0xffffffffu, sc[4 * kk + 1], srcB);
+        const float w0 = __shfl_sync(0xffffffffu, sc[4 * kk + 2], srcB), w1 = __shfl_sync(0xffffffffu, sc[4 * kk + 3], srcB);
+        a[0] = odd ? x1 : x0; a[1] = odd ? y1 : y0; a[2] = odd ? z1 : z0; a[3] = odd ? w1 : w0;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float hi = MODE == 3 ? tf32_hi(a[e]) : a[e];
+          phi[kk][e] = __float_as_uint(hi);
+          plo[kk][e] = __float_as_uint(a[e] - hi);   // the tensor core reads the top 19 bits: truncation costs 2^-21 |p|
+        }
+      }
+    }
+  };
+
+  // Ping-pong: every stage (one per key tile, plus a last one for the final P V) is one bar.sync on the warpgroup's own
+  // barrier before it issues and one bar.arrive on the other's after.  Warpgroup 1 opens with an extra arrive (warpgroup 0
+  // issues first) and skips its arrive after the last stage, so both barriers end complete.  A warpgroup whose rows lie
+  // past the view runs every stage all the same.
+  // Stage j issues S(j) and P(j-1) V(j-1), and the softmax of tile j runs while P(j-1) V(j-1) is in flight.  That P V is
+  // retired at the top of stage j+1 (then O is rescaled and P(j) split): ptxas places a wgmma wait as early as its basic
+  // block allows, so a wait after the softmax in the same block would run before it; the top of the next stage lies
+  // behind the loop's back edge.  The first stage has its own issue branch: a wgmma issued under a condition (j > 0)
+  // that the following wait does not share makes ptxas serialise every wgmma of the kernel.
+  auto finish_pv = [&](int jn) {                                // before stage jn: O += P(jn-1) V(jn-1) can be issued
+    tc::wgmma_wait<0>();                                        // P(jn-2) V(jn-2)
+    tc::fence_acc<64>(o);
+    fence_regs<KS>(phi);
+    fence_regs<KS>(plo);
+    if (jn >= 2) tc::mbar_arrive(v_empty + (jn - 2) % ST);
+    if (jn >= 1) {
+      rescale_o();
+      split_p();
+    }
+  };
+  if (PIPE && wg == 1) named_bar_arrive(PP_BAR + 0, 256);
   int j = 0;
   for (int sg = 0; sg < T; ++sg) {
     if (g.is_cross ? (sg == t) : (sg != t)) continue;
@@ -198,142 +426,43 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
       const int nvalid = cnt - k0;      // keys of this tile that exist
       const int s = j % ST;
       const uint32_t ph = (j / ST) & 1;
-      // ---- S = Q K^T
-      uint32_t qhi[KS][4], qlo[KS][4];
-#pragma unroll
-      for (int kk = 0; kk < KS; ++kk) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          float2 x2 = qraw[kk][e];
-          asm volatile("" : "+f"(x2.x), "+f"(x2.y));           // keeps the split inside the loop (no hoisting)
-          if (F16) {
-            split_pack(x2.x, x2.y, qhi[kk][e], qlo[kk][e]);
-          } else {
-            const float x = x2.x;
-            const float hi = MODE == 3 ? tf32_hi(x) : x;
-            qhi[kk][e] = __float_as_uint(hi);
-            qlo[kk][e] = __float_as_uint(MODE == 3 ? tf32_hi(x - hi) : 0.f);
-          }
-        }
-      }
-      float sc[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) sc[i] = 0.f;
-      tc::mbar_wait(k_full + s, ph);
-      const uint32_t kb = tc::smem_u32(smem + s * TILE);
-      tc::wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < KS; ++kk) {
-        if (F16) {
-          const uint64_t dk = tc::make_sw128_desc(kb + kk * 32);
-          tc::wgmma_f16_rs<64, 0>(sc, qhi[kk], dk);
-          tc::wgmma_f16_rs<64, 0>(sc, qhi[kk], tc::make_sw128_desc(kb + PLANE + kk * 32));
-          tc::wgmma_f16_rs<64, 0>(sc, qlo[kk], dk);
+      if constexpr (PIPE) {
+        finish_pv(j);
+        prep_s();
+        named_bar_sync(PP_BAR + wg, 256);
+        if (j == 0) {
+          issue_s(s, ph);
+          named_bar_arrive(PP_BAR + (wg ^ 1), 256);
+          tc::wgmma_wait<0>();
         } else {
-          const uint32_t off = (kk >> 2) * 8192 + (kk & 3) * 32;
-          const uint64_t dk = tc::make_sw128_desc(kb + off);
-          tc::wgmma_tf32_rs<64>(sc, qhi[kk], dk);
-          if (MODE == 3) {
-            tc::wgmma_tf32_rs<64>(sc, qhi[kk], tc::make_sw128_desc(kb + PLANE + off));
-            tc::wgmma_tf32_rs<64>(sc, qlo[kk], dk);
-          }
+          issue_s(s, ph);
+          issue_pv((j - 1) % ST, ((j - 1) / ST) & 1);
+          named_bar_arrive(PP_BAR + (wg ^ 1), 256);
+          tc::wgmma_wait<1>();
         }
+        retire_s(s);
+        softmax(nvalid);
+      } else {
+        prep_s();
+        issue_s(s, ph);
+        tc::wgmma_wait<0>();
+        retire_s(s);
+        softmax(nvalid);
+        rescale_o();
+        split_p();
+        issue_pv(s, ph);
+        tc::wgmma_wait<0>();
+        retire_pv(s);
       }
-      tc::wgmma_commit();
-      tc::wgmma_wait<0>();
-      tc::fence_acc<64>(sc);
-      tc::mbar_arrive(k_empty + s);
-
-      // ---- online softmax (a row is spread over the four threads of a quad)
-      if (nvalid < BKV) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int key = 8 * i + 2 * tq;
-          if (key >= nvalid) { sc[4 * i] = -INFINITY; sc[4 * i + 2] = -INFINITY; }
-          if (key + 1 >= nvalid) { sc[4 * i + 1] = -INFINITY; sc[4 * i + 3] = -INFINITY; }
-        }
-      }
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        float mx = sc[2 * hh];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * hh], sc[4 * i + 2 * hh + 1]));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-        mx *= scale_l2e;
-        if (mx > m_run[hh] + 8.f) {                           // the same decision in the four threads of the quad
-          const float f = ex2_ftz(m_run[hh] - mx);
-          m_run[hh] = mx;
-          l_run[hh] *= f;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            o[4 * i + 2 * hh] *= f;
-            o[4 * i + 2 * hh + 1] *= f;
-          }
-        }
-        const float nm = 7.f - m_run[hh];
-        float rs = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float p0 = ex2_ftz(fmaf(sc[4 * i + 2 * hh], scale_l2e, nm));
-          const float p1 = ex2_ftz(fmaf(sc[4 * i + 2 * hh + 1], scale_l2e, nm));
-          sc[4 * i + 2 * hh] = p0;
-          sc[4 * i + 2 * hh + 1] = p1;
-          rs += p0 + p1;
-        }
-        l_run[hh] += rs;
-      }
-
-      // ---- P as the register A operand of O += P V
-      uint32_t phi[KS][4], plo[KS][4];
-#pragma unroll
-      for (int kk = 0; kk < KS; ++kk) {
-        if (F16) {
-          // the accumulator layout of keys [16 kk, 16 kk + 16) is the k16 A fragment layout
-#pragma unroll
-          for (int e = 0; e < 4; ++e) split_pack(sc[8 * kk + 2 * e], sc[8 * kk + 2 * e + 1], phi[kk][e], plo[kk][e]);
-        } else {
-          // k8 A fragment: keys tq and tq + 4 of the step, held by quad lanes tq / 2 and 2 + tq / 2
-          float a[4];
-          const bool odd = tq & 1;
-          const float x0 = __shfl_sync(0xffffffffu, sc[4 * kk], srcA), x1 = __shfl_sync(0xffffffffu, sc[4 * kk + 1], srcA);
-          const float y0 = __shfl_sync(0xffffffffu, sc[4 * kk + 2], srcA), y1 = __shfl_sync(0xffffffffu, sc[4 * kk + 3], srcA);
-          const float z0 = __shfl_sync(0xffffffffu, sc[4 * kk], srcB), z1 = __shfl_sync(0xffffffffu, sc[4 * kk + 1], srcB);
-          const float w0 = __shfl_sync(0xffffffffu, sc[4 * kk + 2], srcB), w1 = __shfl_sync(0xffffffffu, sc[4 * kk + 3], srcB);
-          a[0] = odd ? x1 : x0; a[1] = odd ? y1 : y0; a[2] = odd ? z1 : z0; a[3] = odd ? w1 : w0;
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float hi = MODE == 3 ? tf32_hi(a[e]) : a[e];
-            phi[kk][e] = __float_as_uint(hi);
-            plo[kk][e] = __float_as_uint(a[e] - hi);   // the tensor core reads the top 19 bits: truncation costs 2^-21 |p|
-          }
-        }
-      }
-      tc::mbar_wait(v_full + s, ph);
-      const uint32_t vb = tc::smem_u32(smem + C_::OFF_V + s * TILE);
-      tc::wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < KS; ++kk) {
-        if (F16) {
-          const uint64_t dv = tc::make_sw128_desc(vb + kk * 2048);      // 16 keys x 128 B, V key-major (MN-major B)
-          tc::wgmma_f16_rs<64, 1>(o, phi[kk], dv);
-          tc::wgmma_f16_rs<64, 1>(o, phi[kk], tc::make_sw128_desc(vb + PLANE + kk * 2048));
-          tc::wgmma_f16_rs<64, 1>(o, plo[kk], dv);
-        } else {
-          const uint32_t off = (kk >> 2) * 8192 + (kk & 3) * 32;
-          const uint64_t dv = tc::make_sw128_desc(vb + off);
-          tc::wgmma_tf32_rs<64>(o, phi[kk], dv);
-          if (MODE == 3) {
-            tc::wgmma_tf32_rs<64>(o, phi[kk], tc::make_sw128_desc(vb + PLANE + off));
-            tc::wgmma_tf32_rs<64>(o, plo[kk], dv);
-          }
-        }
-      }
-      tc::wgmma_commit();
-      tc::wgmma_wait<0>();
-      tc::fence_acc<64>(o);
-      tc::mbar_arrive(v_empty + s);
     }
+  }
+  if constexpr (PIPE) {                                         // last stage: O += P V of the last tile
+    finish_pv(j);
+    named_bar_sync(PP_BAR + wg, 256);
+    if (j > 0) issue_pv((j - 1) % ST, ((j - 1) / ST) & 1);
+    if (wg == 0) named_bar_arrive(PP_BAR + 1, 256);
+    tc::wgmma_wait<0>();
+    if (j > 0) retire_pv((j - 1) % ST);
   }
 
   // ---- out = O / l
