@@ -11,11 +11,15 @@
 //                       the same 22-bit operands, K = 16 per instruction instead of 8
 // A is split on chip in every mode: it is the register operand of wgmma, so its hi / lo planes never touch shared memory.
 //
-// One CTA computes 128 x BN output tiles with 288 threads:
+// One CTA computes 128 x BN output tiles:
 //   warps 0-3, 4-7   two consumer warpgroups, tile rows [0,64) and [64,128): A fragments from the 128B-swizzled shared
 //                    tile -> hi / lo in registers -> wgmma m64 x BN (B = the W planes, shared-memory descriptors), fp32
-//                    accumulators in registers; then the epilogue straight from the accumulators
-//   warp 8           TMA producer: A [128 x BK] (fp32) and the W planes [BN x 128 B] into a STAGES-deep ring
+//                    accumulators in registers; then the epilogue straight from the accumulators.  With BN = 128 the
+//                    wgmma of k-block kt are issued before the A fragments of kt + 1 are split, so the split runs under
+//                    them (two fragment sets in registers, raised to 232 per thread by setmaxnreg), and the epilogue
+//                    loads its bias / residual operands in batches
+//   warp 8           TMA producer (with BN = 128 warps 8-11, the producer warpgroup, 40 registers): one lane issues the
+//                    TMA loads of A [128 x BK] (fp32) and the W planes [BN x 128 B] into a STAGES-deep ring
 // The tile schedule is static: with `persistent` one CTA per SM walks the tiles (the producer fills the ring for the
 // next tile under the epilogue of the current one), otherwise one tile per CTA.  Both issue the same instructions per
 // tile, so their results are bit-identical.
@@ -31,8 +35,12 @@
 namespace {
 
 constexpr int BM = 128;
-constexpr int NTHREADS = 288;
 constexpr int PRODUCER_WARP = 8;
+// 128-column tiles: 384 threads (warps 8-11 are the producer warpgroup) and setmaxnreg 2 x 232 + 40 = the 504 per-thread
+// registers of one SM sub-partition (one warp of each warpgroup), for the pipelined mainloop.  256-column tiles: 288
+// threads (one producer warp) and the in-order mainloop.
+template <int BN> constexpr int nthreads() { return BN == 128 ? 384 : 288; }
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 enum { W_RAW = 0, W_TF32 = 1, W_F16 = 2 };
 
 template <int BN, int NPASS, int WM>
@@ -89,9 +97,16 @@ __device__ __forceinline__ void split_pack_h(float x0, float x1, uint32_t& hi, u
   hi = *reinterpret_cast<const uint32_t*>(&h);
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
+// A-fragment registers of an issued wgmma stay live (and unchanged) until this point, after the wait that retires it
+__device__ __forceinline__ void fence_afrag(uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) asm volatile("" : "+r"(a[i][e])::"memory");
+}
 
 template <int BN, int NPASS, int WM, bool SCORE>
-__global__ void __launch_bounds__(NTHREADS, 1)
+__global__ void __launch_bounds__(nthreads<BN>(), 1)
 gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                const __grid_constant__ CUtensorMap tmWhi, const __grid_constant__ CUtensorMap tmWlo,
                const __grid_constant__ GArgs g, const __grid_constant__ ScoreTab st) {
@@ -100,6 +115,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   constexpr int BK = C_::BK, STAGES = C_::STAGES, A_BYTES = C_::A_BYTES, W_PLANE = C_::W_PLANE;
   constexpr int STAGE_BYTES = C_::STAGE_BYTES;
   constexpr int KSTEPS = 4;                                   // 4 x (K = 8 tf32 | K = 16 halves) per k-block
+  constexpr bool PIPE = BN == 128;                            // pipelined mainloop (see the consumers)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);   // [STAGES] TMA landed
@@ -132,9 +148,10 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
   __syncthreads();
 
-  if (warp == PRODUCER_WARP) {
+  if (warp >= PRODUCER_WARP) {
     // ================================ TMA producer ================================
-    if (lane == 0) {
+    if (PIPE) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+    if (warp == PRODUCER_WARP && lane == 0) {
       tc::prefetch_tmap(&tmA); tc::prefetch_tmap(&tmA2); tc::prefetch_tmap(&tmWhi); tc::prefetch_tmap(&tmWlo);
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -161,17 +178,17 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 
   // ================================ consumers ================================
+  if (PIPE) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
   const int wg = warp >> 2, wq = warp & 3;
   const int gr = lane >> 2, tq = lane & 3;
   const int row0 = wg * 64 + wq * 16 + gr;                     // tile rows of this thread: row0, row0 + 8
   float acc[BN / 2];
-  uint32_t it = 0;
-  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    int m0, n0, a_row, w_row, prob;
-    decode(tile, m0, n0, a_row, w_row, prob);
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    for (int kt = 0; kt < nk; ++kt, ++it) {
+  // A fragments (hi / lo) of two consecutive k-blocks: k-block kt + 1 is split into one set while the wgmma of kt,
+  // which read the other, are in flight
+  uint32_t ahi0[KSTEPS][4], alo0[KSTEPS][4], ahi1[KSTEPS][4], alo1[KSTEPS][4];
+
+  // wait for ring stage `it`, split its W tile (3xTF32 on raw W) and the A fragments of this thread's rows
+  auto prep = [&](uint32_t it, uint32_t (&ahi)[KSTEPS][4], uint32_t (&alo)[KSTEPS][4]) {
       const int s = it % STAGES;
       tc::mbar_wait(full + s, (it / STAGES) & 1);
       uint8_t* sp = smem + s * STAGE_BYTES;
@@ -192,7 +209,6 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         asm volatile("bar.sync 1, 256;" ::: "memory");
       }
       // A fragments of rows row0 / row0 + 8 from the 128B-swizzled tile: 16-byte chunk c of row r sits at c ^ (r & 7)
-      uint32_t ahi[KSTEPS][4], alo[KSTEPS][4];
       const uint8_t* ar = sp + row0 * 128;
 #pragma unroll
       for (int kk = 0; kk < KSTEPS; ++kk) {
@@ -225,7 +241,10 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       }
-      const uint32_t whi = tc::smem_u32(sp + A_BYTES);
+  };
+  // issue the 4 x 3 (or 4 x 1) wgmma of ring stage `it` as one commit group
+  auto issue = [&](uint32_t it, const uint32_t (&ahi)[KSTEPS][4], const uint32_t (&alo)[KSTEPS][4]) {
+      const uint32_t whi = tc::smem_u32(smem + (it % STAGES) * STAGE_BYTES + A_BYTES);
       tc::wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < KSTEPS; ++kk) {
@@ -247,10 +266,55 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
       tc::wgmma_commit();
+  };
+  auto keep = [&](uint32_t (&ahi)[KSTEPS][4], uint32_t (&alo)[KSTEPS][4]) {
+    fence_afrag(ahi);
+    if (NPASS == 3) fence_afrag(alo);
+  };
+
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    int m0, n0, a_row, w_row, prob;
+    decode(tile, m0, n0, a_row, w_row, prob);
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    // Pipelined mainloop (BN = 128), two k-blocks per trip so that each fragment set has a fixed name.  Every issue is followed by
+    // wait<1> in the same branch: it retires the previous k-block (whose stage is then released and whose fragment
+    // set is refilled), and the split of the next k-block runs while this one's wgmma are on the tensor cores.  The
+    // wait sits before the split because the set it refills is still being read by the retiring wgmma.  The wgmma
+    // sequence, and so every accumulator's sum order, is the same as issuing and retiring one k-block at a time.
+    if constexpr (PIPE) {
+      prep(it, ahi0, alo0);
+      for (int kt = 0; kt < nk; kt += 2) {
+        issue(it + kt, ahi0, alo0);
+        tc::wgmma_wait<1>();
+        keep(ahi1, alo1);
+        if (kt > 0) tc::mbar_arrive(empty + (it + kt - 1) % STAGES);
+        if (kt + 1 < nk) {
+          prep(it + kt + 1, ahi1, alo1);
+          issue(it + kt + 1, ahi1, alo1);
+          tc::wgmma_wait<1>();
+          keep(ahi0, alo0);
+          tc::mbar_arrive(empty + (it + kt) % STAGES);
+          if (kt + 2 < nk) prep(it + kt + 2, ahi0, alo0);
+        }
+      }
       tc::wgmma_wait<0>();
       tc::fence_acc<BN>(acc);
-      tc::mbar_arrive(empty + s);
+      keep(ahi0, alo0);
+      keep(ahi1, alo1);
+      tc::mbar_arrive(empty + (it + nk - 1) % STAGES);
+    } else {                                  // 256-column tiles: 128 accumulators leave no room for a second set
+      for (int kt = 0; kt < nk; ++kt) {
+        prep(it + kt, ahi0, alo0);
+        issue(it + kt, ahi0, alo0);
+        tc::wgmma_wait<0>();
+        tc::fence_acc<BN>(acc);
+        keep(ahi0, alo0);
+        tc::mbar_arrive(empty + (it + kt) % STAGES);
+      }
     }
+    it += nk;
 
     // ================================ epilogue ================================
     if (SCORE) {
@@ -271,46 +335,85 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       continue;
     }
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      const int m = m0 + row0 + 8 * hh;
-      if (m >= g.M) continue;
-#pragma unroll
-      for (int i = 0; i < BN / 8; ++i) {
-        const int n = n0 + 8 * i + 2 * tq;
-        float x0 = g.alpha * acc[4 * i + 2 * hh], x1 = g.alpha * acc[4 * i + 2 * hh + 1];
-        if (g.bias) { x0 += __ldg(g.bias + n); x1 += __ldg(g.bias + n + 1); }
-        if (g.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-        if (g.R) {
-          const float2 r = __ldg(reinterpret_cast<const float2*>(g.R + (long long)m * g.ldr + n));
-          x0 += r.x; x1 += r.y;
-        }
-        if (g.VT && n >= g.vt_col0) {
-          // V^T (and its tf32 lo plane) for the tf32 attention kernel
-          const int slab = m / g.n_pad, ii = m % g.n_pad;
-          const long long off = ((long long)slab * (g.N - g.vt_col0) + (n - g.vt_col0)) * g.n_pad + ii;
-          if (g.VTLO) {
-            const float h0 = tf32_hi(x0), h1 = tf32_hi(x1);
-            g.VT[off] = h0; g.VT[off + g.n_pad] = h1;
-            g.VTLO[off] = tf32_hi(x0 - h0); g.VTLO[off + g.n_pad] = tf32_hi(x1 - h1);
-          } else {
-            g.VT[off] = x0; g.VT[off + g.n_pad] = x1;
-          }
-        } else if (g.KH16 && n >= 256) {
-          // K (columns 256..511) and V (512..767) hi / lo planes in half precision
-          const bool is_v = n >= 512;
-          const long long o = (long long)m * 256 + n - (is_v ? 512 : 256);
-          uint32_t hi, lo;
-          split_pack_h(x0, x1, hi, lo);
-          *reinterpret_cast<uint32_t*>((is_v ? g.VH16 : g.KH16) + o) = hi;
-          *reinterpret_cast<uint32_t*>((is_v ? g.VL16 : g.KL16) + o) = lo;
-        } else if (g.KLO && n >= 256 && n < 512) {
+    // store the finished pair (x0, x1) of row m, columns n, n + 1 in the layout(s) the caller asked for
+    auto put = [&](int m, int n, float x0, float x1) {
+      if (g.VT && n >= g.vt_col0) {
+        // V^T (and its tf32 lo plane) for the tf32 attention kernel
+        const int slab = m / g.n_pad, ii = m % g.n_pad;
+        const long long off = ((long long)slab * (g.N - g.vt_col0) + (n - g.vt_col0)) * g.n_pad + ii;
+        if (g.VTLO) {
           const float h0 = tf32_hi(x0), h1 = tf32_hi(x1);
-          *reinterpret_cast<float2*>(g.C + (long long)m * g.ldc + n) = make_float2(h0, h1);
-          *reinterpret_cast<float2*>(g.KLO + (long long)m * 256 + n - 256) = make_float2(tf32_hi(x0 - h0), tf32_hi(x1 - h1));
+          g.VT[off] = h0; g.VT[off + g.n_pad] = h1;
+          g.VTLO[off] = tf32_hi(x0 - h0); g.VTLO[off + g.n_pad] = tf32_hi(x1 - h1);
         } else {
-          const long long c_row = m + (long long)prob * g.tiles_m * BM;     // split-K: slab of this K slice
-          *reinterpret_cast<float2*>(g.C + c_row * g.ldc + n) = make_float2(x0, x1);
+          g.VT[off] = x0; g.VT[off + g.n_pad] = x1;
+        }
+      } else if (g.KH16 && n >= 256) {
+        // K (columns 256..511) and V (512..767) hi / lo planes in half precision
+        const bool is_v = n >= 512;
+        const long long o = (long long)m * 256 + n - (is_v ? 512 : 256);
+        uint32_t hi, lo;
+        split_pack_h(x0, x1, hi, lo);
+        *reinterpret_cast<uint32_t*>((is_v ? g.VH16 : g.KH16) + o) = hi;
+        *reinterpret_cast<uint32_t*>((is_v ? g.VL16 : g.KL16) + o) = lo;
+      } else if (g.KLO && n >= 256 && n < 512) {
+        const float h0 = tf32_hi(x0), h1 = tf32_hi(x1);
+        *reinterpret_cast<float2*>(g.C + (long long)m * g.ldc + n) = make_float2(h0, h1);
+        *reinterpret_cast<float2*>(g.KLO + (long long)m * 256 + n - 256) = make_float2(tf32_hi(x0 - h0), tf32_hi(x1 - h1));
+      } else {
+        const long long c_row = m + (long long)prob * g.tiles_m * BM;     // split-K: slab of this K slice
+        *reinterpret_cast<float2*>(g.C + c_row * g.ldc + n) = make_float2(x0, x1);
+      }
+    };
+    if constexpr (PIPE) {
+      // The bias and residual operands of ICH column groups are loaded first, all at once, so that their latencies
+      // overlap instead of each standing between the stores of two elements.
+      constexpr int ICH = 8;
+#pragma unroll
+      for (int i0 = 0; i0 < BN / 8; i0 += ICH) {
+        float2 bv[ICH], rv[ICH][2];
+#pragma unroll
+        for (int c = 0; c < ICH; ++c) {
+          const int n = n0 + 8 * (i0 + c) + 2 * tq;
+          bv[c] = g.bias ? make_float2(__ldg(g.bias + n), __ldg(g.bias + n + 1)) : make_float2(0.f, 0.f);
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int m = m0 + row0 + 8 * hh;
+            rv[c][hh] = g.R && m < g.M ? __ldg(reinterpret_cast<const float2*>(g.R + (long long)m * g.ldr + n))
+                                       : make_float2(0.f, 0.f);
+          }
+        }
+#pragma unroll
+        for (int c = 0; c < ICH; ++c) {
+          const int i = i0 + c, n = n0 + 8 * i + 2 * tq;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int m = m0 + row0 + 8 * hh;
+            if (m >= g.M) continue;
+            float x0 = g.alpha * acc[4 * i + 2 * hh], x1 = g.alpha * acc[4 * i + 2 * hh + 1];
+            if (g.bias) { x0 += bv[c].x; x1 += bv[c].y; }
+            if (g.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+            if (g.R) { x0 += rv[c][hh].x; x1 += rv[c][hh].y; }
+            put(m, n, x0, x1);
+          }
+        }
+      }
+    } else {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int m = m0 + row0 + 8 * hh;
+        if (m >= g.M) continue;
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i) {
+          const int n = n0 + 8 * i + 2 * tq;
+          float x0 = g.alpha * acc[4 * i + 2 * hh], x1 = g.alpha * acc[4 * i + 2 * hh + 1];
+          if (g.bias) { x0 += __ldg(g.bias + n); x1 += __ldg(g.bias + n + 1); }
+          if (g.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+          if (g.R) {
+            const float2 r = __ldg(reinterpret_cast<const float2*>(g.R + (long long)m * g.ldr + n));
+            x0 += r.x; x1 += r.y;
+          }
+          put(m, n, x0, x1);
         }
       }
     }
@@ -327,7 +430,7 @@ int launch_wg(const CUtensorMap* tA, const CUtensorMap* tA2, const CUtensorMap* 
   cudaFuncSetAttribute(gemm_wg_kernel<BN, NPASS, WM, SCORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES);
   const int n_sm = mvm_dev_info().n_sm;
   const int grid = (persistent && n_tiles > n_sm) ? n_sm : (int)n_tiles;
-  gemm_wg_kernel<BN, NPASS, WM, SCORE><<<grid, NTHREADS, C_::SMEM_BYTES, stream>>>(*tA, *tA2, *tWhi, *tWlo, g, st);
+  gemm_wg_kernel<BN, NPASS, WM, SCORE><<<grid, nthreads<BN>(), C_::SMEM_BYTES, stream>>>(*tA, *tA2, *tWhi, *tWlo, g, st);
   MVM_CHECK_LAUNCH();
   return MVM_OK;
 }
