@@ -173,7 +173,7 @@ int mvm_matcher_forward_ex(const mvm_matcher_weights* w, int batch, int n_views,
   if (opt) o = *opt; else mvm_matcher_options_default(&o);
   MVM_REQUIRE(o.math_mode == 0 || o.math_mode == 1 || o.math_mode == 3);
   MVM_REQUIRE(o.sinkhorn_variant >= 0 && o.sinkhorn_variant <= 4);
-  MVM_REQUIRE(w && counts && kpts && kscores && desc && pairs && workspace);
+  MVM_REQUIRE(w && counts && kpts && kscores && desc && pairs && workspace && sinkhorn_iters >= 1);
   MVM_REQUIRE(batch >= 1 && n_views >= 2 && n_views <= MVM_MAX_VIEWS);
   MVM_REQUIRE(n_pad >= 64 && n_pad % 64 == 0);
   MVM_REQUIRE(w->n_layers >= 0 && w->n_layers <= MVM_MAX_LAYERS);

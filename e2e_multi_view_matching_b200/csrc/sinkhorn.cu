@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(1024) sinkhorn_ref_kernel(SinkhornTable tab, i
 
 int launch_sinkhorn_ref(const SinkhornTable& tab, int batch, float bin_score, int iters,
                         float* ws, cudaStream_t stream) {
-  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1);
+  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1 && iters >= 1);
   sinkhorn_ref_kernel<<<tab.n_pairs * batch, 1024, 0, stream>>>(tab, batch, bin_score, iters, ws);
   MVM_CHECK_LAUNCH();
   return MVM_OK;
@@ -244,7 +244,7 @@ __global__ void __launch_bounds__(1024, 1) sinkhorn_smem_kernel(PairTable tab, S
 int launch_sinkhorn_log(const SinkhornTable& tab, int batch, float bin_score, int iters, float* ws,
                         cudaStream_t stream) {
   MvmProfScope prof__(MVM_TAG_SINKHORN, stream);
-  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1);
+  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1 && iters >= 1);
   const int n_sm = mvm_dev_info().n_sm;
   const size_t max_smem = mvm_dev_info().max_smem;
   mvm_once_per_device(MVM_ONCE_SINKHORN_LOG, [&] {

@@ -33,6 +33,8 @@ constexpr float ABSORB_HI = 2980.958f;     // e^8
 constexpr float ABSORB_LO = 3.3546263e-4f; // e^-8
 constexpr int CL_ROWS = 64;                // rows of K~ per CTA
 constexpr int CL_MAXN = 1024;              // columns
+constexpr int CL_CRECV = CL_MAXN + 4 + 16; // floats of the crecv region: C * CS <= 1040 for every C
+constexpr int CL_MERGE_COLS = 3;           // columns of its slice one thread of the owner merges: 3 x 512 >= 1025 (C = 1)
 
 __device__ __forceinline__ unsigned cluster_ctarank() {
   unsigned r;
@@ -179,7 +181,7 @@ constexpr int OFF_KB = OFF_B + CL_VEC;                // [n+1]  exp(v~_j): dustb
 constexpr int OFF_VT = OFF_KB + CL_VEC;               // [n+1]  absorbed column potentials v~_j
 constexpr int OFF_COLPART = OFF_VT + CL_VEC;          // [4][1024] column partials of the 4 row groups
 constexpr int OFF_CRECV = OFF_COLPART + 4 * CL_MAXN;  // [C][CS] partials pushed by the peers for my column slice
-constexpr int OFF_ROWPART = OFF_CRECV + CL_MAXN + 4 + 16;   // [8][64] row partials of the 8 column strips
+constexpr int OFF_ROWPART = OFF_CRECV + CL_CRECV;     // [8][64] row partials of the 8 column strips
 constexpr int OFF_A = OFF_ROWPART + 8 * CL_ROWS;      // [64] row scalings a_i, a[64] = dustbin row
 constexpr int OFF_UT = OFF_A + CL_ROWS + 4;           // [64] absorbed row potentials u~_i
 constexpr int OFF_E = OFF_UT + CL_ROWS;               // [64] exp(alpha + u~_i): dustbin column of K~ / kb_n
@@ -202,6 +204,7 @@ __global__ void __launch_bounds__(1024 / RG, 1) sinkhorn_cl_kernel(PairTable tab
   extern __shared__ __align__(16) float smem[];
   constexpr int RS = 16 - RR;
   constexpr int NW = 32 / RG;                       // warps per CTA
+  constexpr int NT = 32 * NW;                       // threads per CTA
   const int C = cfg.C;
   const unsigned c = cluster_ctarank();
   const int prob = blockIdx.x / C;
@@ -505,16 +508,22 @@ __global__ void __launch_bounds__(1024 / RG, 1) sinkhorn_cl_kernel(PairTable tab
       }
     }
     T_MARK(3);
-    // ---- the owner of column j adds the C partials in rank order: b_j = nu_j / (sum_g c_j^g + kb_j a_m) ----
-    if (tid < owned) {       // CS <= 1024: one column per thread
+    // ---- the owner of column j adds the C partials in rank order: b_j = nu_j / (sum_g c_j^g + kb_j a_m).  A slice
+    // can be wider than the CTA (CS = n + 1 for C = 1): thread tid merges columns tid, tid + NT, ... of it.  The loop
+    // bound is what cl_partition_ok checks before the launch: change the two together ----
+    if (tid < owned) {
       mbar_wait(mbarA, ph);
-      const int t = tid, j = (int)c * CS + t;
       const float am = a_s[CL_ROWS];
-      float s = 0.f;
-      for (int g = 0; g < C; ++g) s += crecv[g * CS + t];
-      const float bj = (j < n ? nu : nu_bin) / (s + kb_s[j] * am);
-      for (int g = 0; g < C; ++g)
-        st_async_f32(mapa_u32(b_addr + (unsigned)(j * 4), (unsigned)g), bj, mapa_u32(mbarB, (unsigned)g));
+#pragma unroll 1
+      for (int k = 0; k < CL_MERGE_COLS; ++k) {
+        const int t = tid + k * NT, j = (int)c * CS + t;
+        if (t >= owned) break;
+        float s = 0.f;
+        for (int g = 0; g < C; ++g) s += crecv[g * CS + t];
+        const float bj = (j < n ? nu : nu_bin) / (s + kb_s[j] * am);
+        for (int g = 0; g < C; ++g)
+          st_async_f32(mapa_u32(b_addr + (unsigned)(j * 4), (unsigned)g), bj, mapa_u32(mbarB, (unsigned)g));
+      }
     }
     T_MARK(4);
     // all n+1 scalings of this iteration have landed in b_s.  One warp polls, the others sleep in the barrier: 32
@@ -587,18 +596,29 @@ int sinkhorn_cluster_size(int max_m, int max_n) {
   return C;
 }
 
+// The column partition sinkhorn_cl_kernel relies on for an n-column problem on C CTAs of 1024 / rg threads.  Each
+// iteration waits for the partials and the b_j of every column, so a column that no thread pushes or merges would
+// leave the kernel waiting forever: such a shape is refused before the launch.
+static bool cl_partition_ok(int n, int C, int rg) {
+  const int nt = 1024 / rg, CS = (n + 1 + C - 1) / C;
+  return n <= rg * nt                      // the push loop j = tid + q * nt, q < rg, reaches every column j < n
+         && CS <= CL_MERGE_COLS * nt       // the owner merge has a thread for every column of its slice
+         && C * CS <= CL_CRECV;            // the C partials of a slice fit crecv
+}
+
 int launch_sinkhorn_cluster(const SinkhornTable& tab, int batch, float bin_score, int iters, int C,
                             cudaStream_t stream, int rr) {
-  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1);
+  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1 && iters >= 1);
   MVM_REQUIRE(C == 1 || C == 2 || C == 4 || C == 8 || C == 16);
-  int max_n = 0;
-  for (int p = 0; p < tab.n_pairs; ++p) {
-    MVM_REQUIRE(tab.m[p] >= 1 && tab.n[p] >= 1 && tab.n[p] <= CL_MAXN && tab.m[p] <= C * CL_ROWS);
-    max_n = tab.n[p] > max_n ? tab.n[p] : max_n;
-  }
   if (rr == 0) rr = CL_DEFAULT;
   MVM_REQUIRE(rr == 6 || rr == 8 || rr == 16);      // 16 = two row groups per warp (512 threads), 8 register rows each
   const int rg = rr == 16 ? 2 : 1;
+  int max_n = 0;
+  for (int p = 0; p < tab.n_pairs; ++p) {
+    MVM_REQUIRE(tab.m[p] >= 1 && tab.n[p] >= 1 && tab.n[p] <= CL_MAXN && tab.m[p] <= C * CL_ROWS);
+    MVM_REQUIRE(cl_partition_ok(tab.n[p], C, rg));
+    max_n = tab.n[p] > max_n ? tab.n[p] : max_n;
+  }
   const size_t smem = cl_smem_bytes(max_n, 16 - (rr == 16 ? 8 : rr));
   auto kern = rr == 16 ? (g_sink_timing ? sinkhorn_cl_kernel<8, 2, true> : sinkhorn_cl_kernel<8, 2, false>)
               : rr == 8 ? sinkhorn_cl_kernel<8, 1, false>

@@ -229,7 +229,7 @@ extern "C" void mvm_debug_set_sinkhorn_timing(long long* p) { g_sink_timing = p;
 // with one row group per warp (1024 threads; 8 / 6 register rows), 4 = cluster kernel with two row groups per warp.
 int launch_sinkhorn(const SinkhornTable& tab, int batch, float bin_score, int iters, float* ws,
                     cudaStream_t stream, int variant) {
-  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1);
+  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1 && iters >= 1);
   int mm = 0, mn = 0;
   for (int p = 0; p < tab.n_pairs; ++p) {
     mm = tab.m[p] > mm ? tab.m[p] : mm;
@@ -246,7 +246,7 @@ int launch_sinkhorn(const SinkhornTable& tab, int batch, float bin_score, int it
 
 int launch_sinkhorn_multicta(const SinkhornTable& tab, int batch, float bin_score, int iters, float* ws,
                              cudaStream_t stream) {
-  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1);
+  MVM_REQUIRE(tab.n_pairs >= 1 && tab.n_pairs <= MVM_MAX_PAIRS && batch >= 1 && iters >= 1);
   MvmProfScope prof__(MVM_TAG_SINKHORN, stream);
   const int n_sm = mvm_dev_info().n_sm;
   const size_t max_smem = mvm_dev_info().max_smem;

@@ -203,7 +203,9 @@ int mvm_attention_h3(const float* qkv, const void* kh, const void* kl, const voi
  * mvm_log_optimal_transport is the production kernel (shared-memory-resident, stabilised scaling
  * domain, FMA inner loops); _logdomain is the same multi-CTA layout iterating in the log domain
  * exactly like the reference; _ref is the one-CTA-per-problem kernel that walks the matrix in
- * L2/HBM (both kept as on-device cross-checks). */
+ * L2/HBM (both kept as on-device cross-checks).
+ * iters: Sinkhorn iterations, >= 1 (the reference runs 100).  Every entry point, and mvm_matcher_forward with
+ * sinkhorn_iters, returns 1 (invalid argument) for iters < 1 without launching anything. */
 size_t mvm_sinkhorn_workspace_floats(int n_pairs, int batch, int n_max);
 int mvm_log_optimal_transport(float* scores, int batch, int m, int n, float bin_score,
                               int iters, float* ws, void* stream);
