@@ -81,27 +81,28 @@ __device__ __forceinline__ void mbar_wait(unsigned mbar, unsigned parity) {
 struct OpSum { __device__ __forceinline__ float operator()(float a, float b) const { return a + b; } };
 struct OpMax { __device__ __forceinline__ float operator()(float a, float b) const { return fmaxf(a, b); } };
 
+// Transposed warp reduction: at the level with lane distance S, value k of lane l (k < H) becomes the sum of values
+// k and k + H over the lane pair (l, l ^ S), the lane with bit S clear keeping the lower half.  The levels
+// S = 16, 8, ... run while H >= 1.  Template recursion with a compile-time H at every level: a loop over the levels
+// with a runtime-halving bound is not unrolled by nvcc, and the partials then live in a local-memory array.
+template <int S, int H, int N, class Op>
+__device__ __forceinline__ void xreduce(float (&p)[N], int lane, Op op) {
+  if constexpr (H >= 1) {
+    const bool hi = lane & S;
+#pragma unroll
+    for (int k = 0; k < H; ++k) {
+      const float send = hi ? p[k] : p[k + H], keep = hi ? p[k + H] : p[k];
+      p[k] = op(keep, __shfl_xor_sync(0xffffffffu, send, S));
+    }
+    xreduce<S / 2, H / 2>(p, lane, op);
+  }
+}
+
 // 8 values per lane, reduced over the 32 lanes in 9 shuffles; afterwards every lane holds the total of value index
 // row8(lane) (the four lanes that differ in bits 0-1 hold the same value).
 template <class Op>
 __device__ __forceinline__ float reduce8(float (&p)[8], int lane, Op op) {
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const bool hi = lane & 16;
-    const float send = hi ? p[k] : p[k + 4], keep = hi ? p[k + 4] : p[k];
-    p[k] = op(keep, __shfl_xor_sync(0xffffffffu, send, 16));
-  }
-#pragma unroll
-  for (int k = 0; k < 2; ++k) {
-    const bool hi = lane & 8;
-    const float send = hi ? p[k] : p[k + 2], keep = hi ? p[k + 2] : p[k];
-    p[k] = op(keep, __shfl_xor_sync(0xffffffffu, send, 8));
-  }
-  {
-    const bool hi = lane & 4;
-    const float send = hi ? p[0] : p[1], keep = hi ? p[1] : p[0];
-    p[0] = op(keep, __shfl_xor_sync(0xffffffffu, send, 4));
-  }
+  xreduce<16, 4>(p, lane, op);
   p[0] = op(p[0], __shfl_xor_sync(0xffffffffu, p[0], 2));
   return op(p[0], __shfl_xor_sync(0xffffffffu, p[0], 1));
 }
@@ -111,50 +112,11 @@ __device__ __forceinline__ int row8(int lane) { return ((lane >> 4) & 1) * 4 + (
 // value index row16(lane) (lanes 2k and 2k+1 hold the same value).
 template <class Op>
 __device__ __forceinline__ float reduce16(float (&p)[16], int lane, Op op) {
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const bool hi = lane & 16;
-    const float send = hi ? p[k] : p[k + 8], keep = hi ? p[k + 8] : p[k];
-    p[k] = op(keep, __shfl_xor_sync(0xffffffffu, send, 16));
-  }
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const bool hi = lane & 8;
-    const float send = hi ? p[k] : p[k + 4], keep = hi ? p[k + 4] : p[k];
-    p[k] = op(keep, __shfl_xor_sync(0xffffffffu, send, 8));
-  }
-#pragma unroll
-  for (int k = 0; k < 2; ++k) {
-    const bool hi = lane & 4;
-    const float send = hi ? p[k] : p[k + 2], keep = hi ? p[k + 2] : p[k];
-    p[k] = op(keep, __shfl_xor_sync(0xffffffffu, send, 4));
-  }
-  {
-    const bool hi = lane & 2;
-    const float send = hi ? p[0] : p[1], keep = hi ? p[1] : p[0];
-    p[0] = op(keep, __shfl_xor_sync(0xffffffffu, send, 2));
-  }
+  xreduce<16, 8>(p, lane, op);
   return op(p[0], __shfl_xor_sync(0xffffffffu, p[0], 1));
 }
 __device__ __forceinline__ int row16(int lane) {
   return ((lane >> 4) & 1) * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-}
-
-// 32 values per lane, reduced over the 32 lanes in 31 shuffles; afterwards lane l holds the total of value index l.
-// All the exchanges of a level are independent (16, 8, 4, 2, 1 of them): the instruction-level parallelism the
-// two-row-groups-per-warp kernel needs with only four warps per scheduler.
-template <class Op>
-__device__ __forceinline__ float reduce32(float (&p)[32], int lane, Op op) {
-#pragma unroll
-  for (int w = 16; w >= 1; w >>= 1) {
-    const bool hi = lane & w;
-#pragma unroll
-    for (int k = 0; k < w; ++k) {
-      const float send = hi ? p[k] : p[k + w], keep = hi ? p[k + w] : p[k];
-      p[k] = op(keep, __shfl_xor_sync(0xffffffffu, send, w));
-    }
-  }
-  return p[0];
 }
 
 // b_j of the thread's four columns; 1 beyond the last column (K~ is 0 there)
@@ -355,18 +317,21 @@ __global__ void __launch_bounds__(1024 / RG, 1) sinkhorn_cl_kernel(PairTable tab
       const float4 b4 = load_b4(b_s, col0, n);
       // column re-absorption is decided on the freshly merged b (identical in every CTA of the cluster)
       cbad = (fmaxf(fmaxf(b4.x, b4.y), fmaxf(b4.z, b4.w)) > ABSORB_HI) | (fminf(fminf(b4.x, b4.y), fminf(b4.z, b4.w)) < ABSORB_LO);
-      if (RG == 2) {
-        // all 32 row partials of the warp in one transposed reduction: lane l ends up with the strip total of row l
-        float part[32];
-#pragma unroll
-        for (int g = 0; g < RG; ++g)
+      if constexpr (RG == 2) {
+        // all 32 row partials of the warp in one transposed reduction (levels 16, 8, 4, 2, 1): lane l ends up with
+        // the strip total of row l.  The first level pairs row i of the two row groups, so it runs as soon as both
+        // dot products exist: 16 partials live instead of 32, next to the 64 K~ registers
+        float part[16];
+        const bool hi16 = lane & 16;
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
-          const float4 k = K_GET(g, i);
-          part[g * 16 + i] = fmaf(k.w, b4.w, fmaf(k.z, b4.z, fmaf(k.y, b4.y, k.x * b4.x)));
+          const float4 k0 = K_GET(0, i), k1 = K_GET(1, i);
+          const float p0 = fmaf(k0.w, b4.w, fmaf(k0.z, b4.z, fmaf(k0.y, b4.y, k0.x * b4.x)));
+          const float p1 = fmaf(k1.w, b4.w, fmaf(k1.z, b4.z, fmaf(k1.y, b4.y, k1.x * b4.x)));
+          part[i] = (hi16 ? p1 : p0) + __shfl_xor_sync(0xffffffffu, hi16 ? p0 : p1, 16);
         }
-        const float v = reduce32(part, lane, OpSum());
-        rowpart[cw * CL_ROWS + rp * 32 + lane] = v;
+        xreduce<8, 8>(part, lane, OpSum());
+        rowpart[cw * CL_ROWS + rp * 32 + lane] = part[0];
       } else {
 #pragma unroll
       for (int h8 = 0; h8 < 2; ++h8) {           // groups of 8 rows: 8 partials live instead of 16
