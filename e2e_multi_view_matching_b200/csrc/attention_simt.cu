@@ -147,9 +147,8 @@ __global__ void __launch_bounds__(256) attention_simt_kernel(const float* __rest
 
 int launch_attention_simt(const float* qkv, float* out, int batch, int n_pad, AttnSegs segs,
                           int is_cross, cudaStream_t stream) {
+  MVM_REQUIRE(n_pad % BQ == 0 && attn_segs_valid(segs, n_pad, is_cross));
   MvmProfScope prof__(MVM_TAG_ATTN, stream);
-  MVM_REQUIRE(n_pad % BQ == 0 && segs.n_views >= 1 && segs.n_views <= 8);
-  MVM_REQUIRE(!is_cross || segs.n_views >= 2);
   const int smem_bytes = SMEM_FLOATS * (int)sizeof(float);
   mvm_once_per_device(MVM_ONCE_ATTN_SIMT, [&] {
     cudaFuncSetAttribute(attention_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);

@@ -9,8 +9,7 @@ extern "C" void mvm_debug_set_attention_timing(long long* buf) { g_attn_dbg = bu
 // qkv [V, n_pad, 768] (q | k | unused-v), vt [V, 256, n_pad] = V^T per head; out [V, n_pad, 256]
 int launch_attention_tc(const float* qkv, const float* vt, float* out, int batch, int n_pad, AttnSegs segs,
                         int is_cross, int n_pass, cudaStream_t stream, const float* klo, const float* vtlo) {
-  MVM_REQUIRE(n_pad % 64 == 0 && segs.n_views >= 1 && segs.n_views <= 8);
-  MVM_REQUIRE(!is_cross || segs.n_views >= 2);
+  MVM_REQUIRE(n_pad % 64 == 0 && attn_segs_valid(segs, n_pad, is_cross));
   MvmProfScope prof__(MVM_TAG_ATTN, stream);
   const int V = batch * segs.n_views;
   const long long rows = (long long)V * n_pad;

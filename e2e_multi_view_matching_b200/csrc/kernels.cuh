@@ -50,6 +50,21 @@ struct AttnSegs {
   int n_views;
   int counts[8];
 };
+// What every attention launch needs of its segments, checked on the host before any CUDA call: 1..8 views, cross
+// attention over at least two, every count in [0, n_pad] (a larger count walks the key loop into the next view's rows),
+// and a source key for every query view that has a query row (without one the softmax denominator is 0: NaN output)
+inline bool attn_segs_valid(const AttnSegs& segs, int n_pad, int is_cross) {
+  if (segs.n_views < 1 || segs.n_views > 8 || (is_cross && segs.n_views < 2)) return false;
+  for (int t = 0; t < segs.n_views; ++t)
+    if (segs.counts[t] < 0 || segs.counts[t] > n_pad) return false;
+  for (int t = 0; t < segs.n_views; ++t) {
+    int keys = 0;
+    for (int s = 0; s < segs.n_views; ++s)
+      if (is_cross ? s != t : s == t) keys += segs.counts[s];
+    if (segs.counts[t] > 0 && keys == 0) return false;
+  }
+  return true;
+}
 // klo / vtlo: tf32 remainder planes of K [rows,256] and V^T (n_pass == 3; K and V^T then hold the rn_tf32 parts)
 int launch_attention_tc(const float* qkv, const float* vt, float* out, int batch, int n_pad, AttnSegs segs,
                         int is_cross, int n_pass, cudaStream_t stream, const float* klo = nullptr,

@@ -177,7 +177,13 @@ int mvm_get_math_mode(void);
 /* Multi-head attention over key/value segments (superglue.py:87-109 with the multi-view
  * cross source of multi_view_matcher.py:92-95).  qkv [n_views_total, n_pad, 768]
  * (q|k|v, head-contiguous); view v attends to its own keys (is_cross = 0) or to all other
- * views of its tuple in ascending order (is_cross = 1).  out [n_views_total, n_pad, 256]. */
+ * views of its tuple in ascending order (is_cross = 1).  out [n_views_total, n_pad, 256].
+ * The three attention entry points below share these conditions, and return 1 (invalid argument) before any CUDA call
+ * when the first three fail: 1 <= n_views <= 8 (cross attention: at least 2); every counts[t] in [0, n_pad]; every
+ * view with counts[t] >= 1 has at least one source key (in cross attention, some other view has a nonzero count).
+ * Rows at and beyond counts[t] of qkv (and of the K / V planes) must be FINITE: masked keys get P = 0, and their V
+ * rows are still multiplied by it (0 x inf = NaN); their values do not otherwise reach rows below the counts.  Output
+ * rows at and beyond counts[t] are unspecified. */
 int mvm_attention(const float* qkv, float* out, int batch, int n_views, int n_pad,
                   const int* counts, int is_cross, void* stream);
 
