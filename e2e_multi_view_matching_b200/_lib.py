@@ -161,6 +161,9 @@ def lib():
     L.mvm_w8pt.restype = C.c_int
     L.mvm_w8pt.argtypes = [_fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, C.c_int, C.c_int, _fp,
                            _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]
+    L.mvm_ransac_essential.restype = C.c_int
+    L.mvm_ransac_essential.argtypes = [_fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, C.c_float, C.c_double, C.c_int,
+                                       C.c_ulonglong, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]
     L.mvm_ba2view.restype = C.c_int
     L.mvm_ba2view.argtypes = [_fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp, _fp, _fp, _fp, _fp, _fp, _fp]
     L.mvm_gather_matches.restype = C.c_int

@@ -1,6 +1,7 @@
-"""Two-view benchmark driver with the reference's flow (eval_pairs.py:130-278) for the `w8pt` and
-`w8pt_ba` modes: pairwise matcher (multi_frame_matching=False, 18 layers, confidence head), weighted
-eight-point, optional two-view bundle adjustment, AUC@5/10/20 as JSON.  Data are synthetic two-view
+"""Two-view benchmark driver with the reference's flow (eval_pairs.py:130-278) for its four modes: pairwise matcher
+(multi_frame_matching=False, 18 layers, confidence head), then weighted eight-point (`w8pt`) or RANSAC + recoverPose on
+the matches above match_threshold 0.02 (`ransac`, eval_pairs.py:152), each optionally followed by the two-view bundle
+adjustment (`w8pt_ba`, `ransac_ba`), AUC@5/10/20 as JSON.  Data are synthetic two-view
 scenes (no datasets offline): 1024 keypoints @ 640x480 ("scannet") or 2048 @ 1600x1200 ("megadepth").
 
     python -m e2e_multi_view_matching_b200.eval_pairs --eval_mode w8pt_ba --n_pairs 64
@@ -18,7 +19,7 @@ from .synthetic import make_state_dict, make_scene_tuple_inputs
 
 def main(argv=None):
     ap = argparse.ArgumentParser()
-    ap.add_argument('--eval_mode', default='w8pt_ba', choices=['w8pt', 'w8pt_ba'])
+    ap.add_argument('--eval_mode', default='w8pt_ba', choices=['ransac', 'ransac_ba', 'w8pt', 'w8pt_ba'])
     ap.add_argument('--dataset', default='scannet', choices=['scannet', 'megadepth', 'yfcc100m'])
     ap.add_argument('--n_pairs', type=int, default=32)
     ap.add_argument('--batch', type=int, default=32)
@@ -47,7 +48,8 @@ def main(argv=None):
         sd = make_state_dict(len(layers), seed=opt.seed, final_proj_gain=12.0, conf_head='score')
         matcher.load_state_dict({k: torch.from_numpy(np.asarray(v)) for k, v in sd.items()})
     matcher = matcher.cuda()
-    pipe = PairPipeline(matcher, eval_mode=opt.eval_mode)
+    match_threshold = 0.02 if 'ransac' in opt.eval_mode else 0.0        # eval_pairs.py:152
+    pipe = PairPipeline(matcher, eval_mode=opt.eval_mode, match_threshold=match_threshold)
     errors, failed = [], 0
     with torch.no_grad():
         for start in range(0, opt.n_pairs, opt.batch):

@@ -2,7 +2,7 @@
 
   MultiViewPipeline.__call__  ==  eval_multi_view.py:152-162 (matcher on a tuple, then
                                   eval_bundle_adjust, eval_multi_view.py:21-68)
-  PairPipeline.__call__       ==  eval_pairs.py:208-267 for the w8pt / w8pt_ba modes
+  PairPipeline.__call__       ==  eval_pairs.py:208-267 for the w8pt / w8pt_ba / ransac / ransac_ba modes
 
 Inputs are the reference's `data` dicts (keypoints{i}, scores{i}, descriptors{i}, image{i}, intr{i},
 ids); there is no numpy hop between matcher and pose, no subprocess and no CSV file.
@@ -89,10 +89,11 @@ class MultiViewPipeline:
 
 
 class PairPipeline:
-    """matcher (pairwise) + w8pt [+ two-view BA] (eval_pairs.py modes `w8pt`, `w8pt_ba`)."""
+    """matcher (pairwise) + w8pt or RANSAC [+ two-view BA] (eval_pairs.py modes `w8pt`, `w8pt_ba`, `ransac`,
+    `ransac_ba`)."""
 
     def __init__(self, matcher: MultiViewMatcher, eval_mode='w8pt_ba', match_threshold=0.0):
-        assert eval_mode in ('w8pt', 'w8pt_ba')
+        assert eval_mode in ('w8pt', 'w8pt_ba', 'ransac', 'ransac_ba')
         self.matcher = matcher
         self.eval_mode = eval_mode
         self.pose = MultiViewPoseEngine(conf_thresh=match_threshold)
@@ -103,6 +104,12 @@ class PairPipeline:
         if state is None:            # a view without keypoints: "cannot compute pose" (eval_pairs.py:258-260)
             return result, None
         intr = [data['intr0'], data['intr1']]
+        if self.eval_mode.startswith('ransac'):
+            pose = self.pose.run(state, intr, global_ba=False, rel_pose_method=self.eval_mode)
+            return result, {'T_021': pose['T_pair'][:, 0], 'success': pose['success'][:, 0],
+                            'inliers': pose['inliers'][:, 0], 'n_inliers': pose['n_inliers'][:, 0],
+                            'ransac_iterations': pose['ransac_iterations'][:, 0], **{k: v for k, v in pose.items()
+                                                                                    if k not in ('inliers', 'n_inliers')}}
         pose = self.pose.run(state, intr, global_ba=False)
         T = pose['T_pair'] if self.eval_mode == 'w8pt_ba' else pose['T_w8pt']
         return result, {'T_021': T[:, 0], 'success': pose['success'][:, 0], **pose}

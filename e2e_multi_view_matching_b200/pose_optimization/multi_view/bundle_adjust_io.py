@@ -14,8 +14,10 @@ same names, same `<dir>` argument, same files -- build.py::build_cli) the unmodi
 `build_dir` at `BUNDLE_ADJUSTMENT_BUILD_DIR`.  `solve()` is the in-process route (no files, no subprocess);
 the batched, device-resident route of the hot path is `pose_engine.MultiViewPoseEngine`.
 
-The RANSAC relative-pose modes (`rel_pose_method="ransac"/"ransac_ba"`) are OpenCV CPU baselines of the
-reference, not part of the accelerated path: they raise NotImplementedError here.
+The RANSAC relative-pose modes (`rel_pose_method="ransac"/"ransac_ba"`) are not wired into the multi-view flow:
+they raise NotImplementedError here.  Their two-view form (estimate_pose, eval_pairs.py's `ransac` / `ransac_ba`) runs
+on the GPU through `models.utils.estimate_pose` and `MultiViewPoseEngine.run(..., rel_pose_method='ransac'|'ransac_ba',
+global_ba=False)`.
 """
 import ctypes as C
 import logging

@@ -24,8 +24,12 @@ def _intr4(intr):
 
 class MultiViewPoseEngine:
     def __init__(self, conf_thresh=0.0, n_iterations_2view=10, max_iterations_ba=50, use_ba_init=True,
-                 min_inliers=20):
+                 min_inliers=20, ransac_thresh=1.0, ransac_conf=0.99999, ransac_max_iters=1000, ransac_seed=0):
         self.conf_thresh = conf_thresh
+        self.ransac_thresh = ransac_thresh           # pixels (eval_pairs.py:229)
+        self.ransac_conf = ransac_conf               # estimate_pose's conf (models/models/utils.py:288)
+        self.ransac_max_iters = ransac_max_iters     # OpenCV's findEssentialMat default
+        self.ransac_seed = ransac_seed
         self.n_it2 = n_iterations_2view
         self.max_it = max_iterations_ba
         self.use_ba_init = use_ba_init
@@ -43,9 +47,18 @@ class MultiViewPoseEngine:
             self._pair_index_key = key
         return self._pair_index_val
 
-    def run(self, state, intr, global_ba=True):
+    def run(self, state, intr, global_ba=True, rel_pose_method='w8pt_ba'):
         """state: MatcherEngine.last of the matcher call; intr: list (per view) of [B,3,3]/[B,4,4]
-        intrinsics.  Returns dict with pairwise poses and (if global_ba) absolute extrinsics."""
+        intrinsics.  Returns dict with pairwise poses and (if global_ba) absolute extrinsics.
+        rel_pose_method: 'w8pt' / 'w8pt_ba' (the same launches: w8pt, then the two-view BA) or the two-view RANSAC
+        modes 'ransac' / 'ransac_ba' (eval_pairs.py:228-243; pairwise poses only, global_ba must be False)."""
+        if rel_pose_method not in ('w8pt', 'w8pt_ba', 'ransac', 'ransac_ba'):
+            raise ValueError('rel_pose_method must be one of w8pt, w8pt_ba, ransac, ransac_ba, not %r' % (rel_pose_method,))
+        if rel_pose_method.startswith('ransac'):
+            if global_ba:
+                raise ValueError('rel_pose_method=%r computes pairwise poses only: call run(..., global_ba=False)'
+                                 % rel_pose_method)
+            return self._run_ransac(state, intr, rel_pose_method == 'ransac_ba')
         lib = _lib.lib()
         kp, counts, n_pad = state['kpts'], state['counts'], state['n_pad']
         pairs, pair_ids = state['pairs'], state['pair_ids']
@@ -112,6 +125,60 @@ class MultiViewPoseEngine:
                        'mvm_multi_view_ba')
             out.update({'extrinsics_tree': extr_tree, 'extrinsics_init': extr0, 'extrinsics': extr, 'ba_iterations': iters, 'ba_cost': cost,
                         'kpts_norm_a': k0n, 'kpts_norm_b': k1n, 'mconf': mconf})
+        return out
+
+    def _run_ransac(self, state, intr, refine):
+        """eval_pairs.py:228-243: estimate_pose (RANSAC + recoverPose) on the valid matches of every pair, then, with
+        refine, the two-view BA on the inliers of that pose weighted by the raw match confidences."""
+        lib = _lib.lib()
+        kp, counts, n_pad = state['kpts'], state['counts'], state['n_pad']
+        pairs, pair_ids = state['pairs'], state['pair_ids']
+        B, T, P = state['batch'], state['n_views'], len(state['pair_ids'])
+        dev = kp.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        i32 = dict(dtype=torch.int32, device=dev)
+        u8 = dict(dtype=torch.uint8, device=dev)
+        BP = B * P
+        mk0 = torch.empty(B, P, n_pad, 2, **f32)
+        mk1 = torch.empty(B, P, n_pad, 2, **f32)
+        mconf = torch.empty(B, P, n_pad, **f32)
+        n_valid = torch.empty(B, P, **i32)
+        cnt = (C.c_int * T)(*counts)
+        sp = _lib.stream_ptr()
+        with torch.cuda.device(dev):
+            _lib.check(lib.mvm_gather_matches(_lib.ptr(kp), T, n_pad, cnt, pairs, P, B, float(self.conf_thresh),
+                                              _lib.ptr(mk0), _lib.ptr(mk1), _lib.ptr(mconf), _lib.ptr(n_valid), sp),
+                       'mvm_gather_matches')
+            i4 = torch.stack([_intr4(k.to(dev)) for k in intr], 1)
+            ia_idx, ib_idx = self._pair_index(pair_ids, dev)
+            ia = i4.index_select(1, ia_idx).contiguous()
+            ib = i4.index_select(1, ib_idx).contiguous()
+            T_r = torch.empty(B, P, 4, 4, **f32)
+            k0n = torch.empty(B, P, n_pad, 2, **f32)
+            k1n = torch.empty(B, P, n_pad, 2, **f32)
+            inl = torch.empty(B, P, n_pad, **u8)
+            n_inl = torch.empty(B, P, **i32)
+            E = torch.empty(B, P, 10, 9, dtype=torch.float64, device=dev)
+            n_mod = torch.empty(B, P, **i32)
+            iters = torch.empty(B, P, **i32)
+            succ = torch.empty(B, P, **u8)
+            _lib.check(lib.mvm_ransac_essential(_lib.ptr(mk0), _lib.ptr(mk1), _lib.ptr(ia), _lib.ptr(ib), BP, n_pad,
+                                                _lib.ptr(n_valid), float(self.ransac_thresh), float(self.ransac_conf),
+                                                int(self.ransac_max_iters), int(self.ransac_seed), _lib.ptr(T_r),
+                                                _lib.ptr(k0n), _lib.ptr(k1n), _lib.ptr(inl), _lib.ptr(n_inl), _lib.ptr(E),
+                                                _lib.ptr(n_mod), _lib.ptr(iters), _lib.ptr(succ), sp),
+                       'mvm_ransac_essential')
+            out = {'T_ransac': T_r, 'T_pair': T_r, 'success': succ.bool(), 'n_matches': n_valid, 'inliers': inl,
+                   'n_inliers': n_inl, 'ransac_iterations': iters, 'E': E, 'n_models': n_mod,
+                   'kpts_a': mk0, 'kpts_b': mk1, 'mconf': mconf, 'kpts_norm_a': k0n, 'kpts_norm_b': k1n}
+            if refine:
+                T_ba = torch.empty(B, P, 4, 4, **f32)
+                valid = torch.empty(B, P, **u8)
+                pts = torch.empty(BP * n_pad * 3, dtype=torch.float64, device=dev)
+                _lib.check(lib.mvm_ba2view(_lib.ptr(k0n), _lib.ptr(k1n), _lib.ptr(mconf), _lib.ptr(T_r), BP, n_pad,
+                                           int(self.n_it2), _lib.ptr(T_ba), _lib.ptr(valid), _lib.ptr(pts), None,
+                                           _lib.ptr(n_valid), _lib.ptr(inl), sp), 'mvm_ba2view')
+                out.update({'T_pair': T_ba, 'valid_ba': valid.bool()})
         return out
 
 

@@ -252,6 +252,32 @@ int mvm_w8pt(const float* kpts0, const float* kpts1, const float* intr0, const f
              float* conf_norm, unsigned char* pos_depth_mask, unsigned char* inliers,
              float* F_out, const int* n_valid, unsigned char* success, void* stream);
 
+/* estimate_pose (models/models/utils.py:288-312): OpenCV's findEssentialMat(method=RANSAC) + recoverPose, restated
+ * (tests/ransac_oracle.py), one CTA per batch element, fp64 on chip, the whole batch in one launch.
+ *   kpts0/1 [B,N,2] pixels (kpts1 already gathered by the matches), intr0/1 [B,4] = fx,fy,cx,cy, n_valid [B] (device,
+ *   may be NULL = N): effective matches per item.  Points normalised in fp64 as (k - c) / f; inlier threshold
+ *   thresh_px / mean(fx0, fy1, fx0, fy1) on OpenCV's error (x2'Ex1)^2 / (Ex1_0^2 + Ex1_1^2 + E'x2_0^2 + E'x2_1^2),
+ *   rounded to float; prob / max_iters: OpenCV's confidence and iteration cap (the reference: 0.99999, 1000).
+ *   Samples come from splitmix64(seed, hypothesis, draw, attempt), independent of the batch position.
+ * Outputs: T021 [B,16] row-major 4x4 (R | unit t of recoverPose; identity when success = 0); kpts{0,1}_norm [B,N,2];
+ * inliers [B,N] bytes = the mask recoverPose leaves (RANSAC inliers at depth 0..50 in both cameras: estimate_pose's
+ * positional 1e9 is the R output of the recoverPose overload it resolves to, so OpenCV's fixed threshold of 50
+ * applies); n_inliers [B] its
+ * count; E_out [B,10,9] doubles = findEssentialMat's E (unit Frobenius norm, largest entry positive): the chosen
+ * model (n_models = 1) for n_valid > 5, every solution of the five-point problem (n_models <= 10) for n_valid == 5;
+ * iterations [B] = hypotheses the sequential RANSAC loop consumed (0 for n_valid <= 5); success [B] = 0 for fewer
+ * than 5 matches, when no model reaches 5 inliers, or when no match passes recoverPose (the reference's None).
+ * With n_valid == 5 the pose is that of the first solution with a nonzero count (each recoverPose call keeps only the
+ * matches the previous one left, so no later count can be larger), and the solutions come in ascending order of the
+ * solver's hidden variable, not in OpenCV's order: the 5-match pose is not the reference's.
+ * Returns 1 (invalid argument) before launching when a pointer other than n_valid is NULL, batch < 1, n < 1,
+ * n > 2048 (the matches of a pair are held in shared memory), thresh_px <= 0, prob outside [0, 1] or max_iters < 1. */
+int mvm_ransac_essential(const float* kpts0, const float* kpts1, const float* intr0, const float* intr1,
+                         int batch, int n, const int* n_valid, float thresh_px, double prob, int max_iters,
+                         unsigned long long seed, float* T021, float* kpts0_norm, float* kpts1_norm,
+                         unsigned char* inliers, int* n_inliers, double* E_out, int* n_models,
+                         int* iterations, unsigned char* success, void* stream);
+
 /* run_bundle_adjust_2_view -> BundleAdjustGaussNewton2View.run
  * (estimate_relative_pose.py:138-143, bundle_adjust_gauss_newton_2_view.py:127-201):
  * LM with the reference's schedule, Schur-complement step, one CTA per batch element.
