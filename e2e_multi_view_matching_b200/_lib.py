@@ -116,6 +116,11 @@ def lib():
         C.POINTER(MatcherWeights), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), _fp, _fp, _fp,
         C.c_float, C.c_float, C.c_int, C.c_float, C.POINTER(PairIO), C.c_int, _fp, C.c_size_t,
         C.POINTER(MatcherOptions), _fp]
+    L.mvm_matcher_forward_views.restype = C.c_int
+    L.mvm_matcher_forward_views.argtypes = [
+        C.POINTER(MatcherWeights), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), _fp, _fp, _fp,
+        C.POINTER(C.c_float), C.c_int, C.c_float, C.POINTER(PairIO), C.c_int, _fp, C.c_size_t,
+        C.POINTER(MatcherOptions), _fp]
     for name in ('mvm_debug_set_score_kernel', 'mvm_debug_set_gemm_tile', 'mvm_debug_set_gemm_kernel',
                  'mvm_debug_set_attention_split', 'mvm_debug_set_gemm_split', 'mvm_debug_set_attention_h3_variant'):
         getattr(L, name).restype = None

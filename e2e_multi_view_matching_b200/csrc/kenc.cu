@@ -1,12 +1,20 @@
 // Keypoint encoder front (3->32->64->128 with folded BN + ReLU) and the channel-first ->
-// point-major descriptor transpose.  Reference: normalize_keypoints superglue.py:65-72,
+// point-major descriptor transpose.  Keypoints are normalised by the image size of their own view slot (a pair may
+// mix portrait and landscape images).  Reference: normalize_keypoints superglue.py:65-72,
 // KeypointEncoder multi_view_matcher.py:24-37.  The 128->256->256 tail runs as GEMMs.
+#include "../../include/mvm_b200.h"
 #include "common.cuh"
 #include "kernels.cuh"
 
 namespace {
 
 constexpr int PTS = 64;  // points per block
+
+// normalize_keypoints (superglue.py:65-72) per view slot: x_n = (x - cx) / scale, y_n = (y - cy) / scale
+struct KencViews {
+  float cx[MVM_MAX_VIEWS], cy[MVM_MAX_VIEWS], scale[MVM_MAX_VIEWS];
+  int n_views, n_pad;
+};
 
 // Shared-memory layout (floats).  Weights are staged k-major ([k][c]) and activations point-minor ([k][p]) so
 // that a thread's register tile (4 points x 4 or 8 channels) is fed by float4 loads that are broadcast across
@@ -24,7 +32,7 @@ __global__ void __launch_bounds__(256) kenc_front_kernel(const float* __restrict
                                                          const float* w1, const float* b1,
                                                          const float* w2, const float* b2,
                                                          float* __restrict__ h3, int n_points,
-                                                         float cx, float cy, float scale) {
+                                                         const KencViews vt) {
   extern __shared__ float sm[];
   float* s_w1 = sm + OFF_W1; float* s_w2 = sm + OFF_W2;
   float* s_h1 = sm + OFF_H1; float* s_h2 = sm + OFF_H2; float* s_in = sm + OFF_IN;
@@ -38,6 +46,12 @@ __global__ void __launch_bounds__(256) kenc_front_kernel(const float* __restrict
     const int p = p0 + tid;
     float x = 0.f, y = 0.f, sc = 0.f;
     if (p < n_points) {
+      // the slot's entry by compare-and-select: a dynamic index into the parameter table would go through local memory
+      const int v = (p / vt.n_pad) % vt.n_views;
+      float cx = vt.cx[0], cy = vt.cy[0], scale = vt.scale[0];
+#pragma unroll
+      for (int i = 1; i < MVM_MAX_VIEWS; ++i)
+        if (i == v) { cx = vt.cx[i]; cy = vt.cy[i]; scale = vt.scale[i]; }
       x = (kpts[2 * p] - cx) / scale;
       y = (kpts[2 * p + 1] - cy) / scale;
       sc = kscores[p];
@@ -129,16 +143,24 @@ __global__ void transpose_cn_kernel(const float* __restrict__ in, float* __restr
 }  // namespace
 
 int launch_kenc_front(const float* kpts, const float* kscores, const float* const* w,
-                      const float* const* b, float* h3, int n_points, float img_w, float img_h,
-                      cudaStream_t stream) {
+                      const float* const* b, float* h3, int n_points, const float* view_wh, int n_views,
+                      int n_pad, cudaStream_t stream) {
+  MVM_REQUIRE(view_wh && n_views >= 1 && n_views <= MVM_MAX_VIEWS && n_pad >= 1);
   MvmProfScope prof__(MVM_TAG_KENC, stream);
-  const float scale = 0.7f * fmaxf(img_w, img_h);
+  KencViews vt = {};
+  vt.n_views = n_views;
+  vt.n_pad = n_pad;
+  for (int t = 0; t < n_views; ++t) {
+    const float img_w = view_wh[2 * t], img_h = view_wh[2 * t + 1];
+    vt.cx[t] = img_w * 0.5f;
+    vt.cy[t] = img_h * 0.5f;
+    vt.scale[t] = 0.7f * fmaxf(img_w, img_h);
+  }
   mvm_once_per_device(MVM_ONCE_KENC, [&] {
     cudaFuncSetAttribute(kenc_front_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, KENC_SMEM);
   });
   kenc_front_kernel<<<mvm_div_up(n_points, PTS), 256, KENC_SMEM, stream>>>(
-      kpts, kscores, w[0], b[0], w[1], b[1], w[2], b[2], h3, n_points, img_w * 0.5f, img_h * 0.5f,
-      scale);
+      kpts, kscores, w[0], b[0], w[1], b[1], w[2], b[2], h3, n_points, vt);
   MVM_CHECK_LAUNCH();
   return MVM_OK;
 }

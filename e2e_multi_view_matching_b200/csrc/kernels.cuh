@@ -22,9 +22,10 @@ struct PairTable {
 };
 typedef PairTable SinkhornTable;
 
+// view_wh: host float[n_views][2], (width, height) of each view slot; row r belongs to slot (r / n_pad) % n_views
 int launch_kenc_front(const float* kpts, const float* kscores, const float* const* w,
-                      const float* const* b, float* h3, int n_points, float img_w, float img_h,
-                      cudaStream_t stream);
+                      const float* const* b, float* h3, int n_points, const float* view_wh, int n_views,
+                      int n_pad, cudaStream_t stream);
 int launch_transpose_cn(const float* in, float* out, int n_views_total, int C, int n_pad,
                         cudaStream_t stream);
 

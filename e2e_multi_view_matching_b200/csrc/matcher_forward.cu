@@ -168,12 +168,23 @@ int mvm_matcher_forward_ex(const mvm_matcher_weights* w, int batch, int n_views,
                            const float* desc, float img_w, float img_h, int sinkhorn_iters,
                            float match_threshold, const mvm_pair_io* pairs, int n_pairs,
                            void* workspace, size_t workspace_bytes, const mvm_matcher_options* opt, void* stream_) {
+  float view_wh[MVM_MAX_VIEWS][2];
+  for (int t = 0; t < MVM_MAX_VIEWS; ++t) { view_wh[t][0] = img_w; view_wh[t][1] = img_h; }
+  return mvm_matcher_forward_views(w, batch, n_views, n_pad, counts, kpts, kscores, desc, &view_wh[0][0], sinkhorn_iters,
+                                   match_threshold, pairs, n_pairs, workspace, workspace_bytes, opt, stream_);
+}
+
+int mvm_matcher_forward_views(const mvm_matcher_weights* w, int batch, int n_views, int n_pad,
+                              const int* counts, const float* kpts, const float* kscores,
+                              const float* desc, const float* view_wh, int sinkhorn_iters,
+                              float match_threshold, const mvm_pair_io* pairs, int n_pairs,
+                              void* workspace, size_t workspace_bytes, const mvm_matcher_options* opt, void* stream_) {
   cudaStream_t s = (cudaStream_t)stream_;
   mvm_matcher_options o;
   if (opt) o = *opt; else mvm_matcher_options_default(&o);
   MVM_REQUIRE(o.math_mode == 0 || o.math_mode == 1 || o.math_mode == 3);
   MVM_REQUIRE(o.sinkhorn_variant >= 0 && o.sinkhorn_variant <= 4);
-  MVM_REQUIRE(w && counts && kpts && kscores && desc && pairs && workspace && sinkhorn_iters >= 1);
+  MVM_REQUIRE(w && counts && kpts && kscores && desc && view_wh && pairs && workspace && sinkhorn_iters >= 1);
   MVM_REQUIRE(batch >= 1 && n_views >= 2 && n_views <= MVM_MAX_VIEWS);
   MVM_REQUIRE(n_pad >= 64 && n_pad % 64 == 0);
   MVM_REQUIRE(w->n_layers >= 0 && w->n_layers <= MVM_MAX_LAYERS);
@@ -200,7 +211,7 @@ int mvm_matcher_forward_ex(const mvm_matcher_weights* w, int batch, int n_views,
 
   // keypoint encoder + descriptor add (multi_view_matcher.py:265-269)
   MVM_TRY(launch_transpose_cn(desc, ws.DT, V, 256, n_pad, s));
-  MVM_TRY(launch_kenc_front(kpts, kscores, w->kenc_w, w->kenc_b, ws.H3, rows, img_w, img_h, s));
+  MVM_TRY(launch_kenc_front(kpts, kscores, w->kenc_w, w->kenc_b, ws.H3, rows, view_wh, n_views, n_pad, s));
   MVM_TRY(run_gemm(cx, make_gemm(ws.H3, 128, w->kenc_w[3], 128, w->kenc_b[3], ws.H4, 256, rows, 256, 1), s));
   {
     GemmDesc g = make_gemm(ws.H4, 256, w->kenc_w[4], 256, w->kenc_b[4], ws.X, 256, rows, 256, 0);

@@ -9,8 +9,10 @@
 //                         output channels, input patch and weights staged in shared memory per 16-channel slice,
 //                         2 pixels x 32 channels of accumulators per thread.  (First cut of this row: an implicit-GEMM
 //                         tensor-core version is the next step; the 1x1 heads already run on the tensor cores.)
-//   sp_maxpool2_kernel    2x2 / stride 2 max pooling
+//   sp_maxpool2_kernel    2x2 / stride 2 max pooling; odd sizes floor like nn.MaxPool2d(2, 2) (the last row / column
+//                         is dropped), so after three pools the coarse map is h = floor(H/8) x w = floor(W/8)
 //   sp_scores_kernel      convPb (1x1, 256 -> 65) + softmax over the 65 bins + depth-to-space into the [8h, 8w] score map
+//                         (rows / columns of the image past 8h / 8w have no score, as in the reference)
 //   sp_maxpool_rows/cols  separable (2r+1)^2 max filter used by simple_nms (superpoint.py:47-63)
 //   sp_nms_step kernels   the reference's three-round suppression, statement for statement
 //   sp_l2norm_kernel      per-pixel L2 normalisation of the dense descriptors (:216)
@@ -293,7 +295,7 @@ int mvm_superpoint_dense(const mvm_superpoint_weights* wt, const float* image, i
                          void* stream_) {
   cudaStream_t s = (cudaStream_t)stream_;
   MVM_REQUIRE(wt && image && scores_nms && dense_desc && workspace);
-  MVM_REQUIRE(batch >= 1 && height % 8 == 0 && width % 8 == 0 && height >= 16 && width >= 16 && nms_radius >= 0);
+  MVM_REQUIRE(batch >= 1 && height >= 16 && width >= 16 && nms_radius >= 0);
   if (workspace_bytes < mvm_superpoint_workspace_bytes(batch, height, width)) return MVM_ERR_WORKSPACE;
   MvmProfScope prof__(MVM_TAG_MISC, s);
   const size_t px = (size_t)batch * height * width;
@@ -319,19 +321,20 @@ int mvm_superpoint_dense(const mvm_superpoint_weights* wt, const float* image, i
   SP_TRY(conv3x3(A, wt->w[8], wt->b[8], Bf, batch, H, W, 128, 256, 1, s));       // cPa
   sp_scores_kernel<<<(int)((cpx * 32 + 255) / 256), 256, 0, s>>>(Bf, wt->w_pb, wt->b_pb, P0, batch, H, W);
   MVM_CHECK_LAUNCH();
-  // simple_nms (:47-63)
+  // simple_nms (:47-63) on the [8h, 8w] score map
+  const int hs = 8 * H, ws = 8 * W;
   {
-    const long long n = (long long)px;
+    const long long n = (long long)batch * hs * ws;
     const int blocks = mvm_dev_info().n_sm * 4;
-    SP_TRY(maxfilter(P0, P4, P1, batch, height, width, nms_radius, s));          // P1 = max_pool(scores)
+    SP_TRY(maxfilter(P0, P4, P1, batch, hs, ws, nms_radius, s));                  // P1 = max_pool(scores)
     sp_nms_init_kernel<<<blocks, 256, 0, s>>>(P0, P1, P2, n);                    // P2 = max_mask
     MVM_CHECK_LAUNCH();
     for (int it = 0; it < 2; ++it) {
-      SP_TRY(maxfilter(P2, P4, P1, batch, height, width, nms_radius, s));        // P1 = max_pool(max_mask)  (> 0 = supp_mask)
+      SP_TRY(maxfilter(P2, P4, P1, batch, hs, ws, nms_radius, s));                // P1 = max_pool(max_mask)  (> 0 = supp_mask)
       sp_nms_supp_kernel<<<blocks, 256, 0, s>>>(P0, P1, P3, n);                  // P3 = supp_scores
       MVM_CHECK_LAUNCH();
       float* pooled_supp = scores_nms;                                           // scratch until the final write
-      SP_TRY(maxfilter(P3, P4, pooled_supp, batch, height, width, nms_radius, s));
+      SP_TRY(maxfilter(P3, P4, pooled_supp, batch, hs, ws, nms_radius, s));
       sp_nms_update_kernel<<<blocks, 256, 0, s>>>(P3, pooled_supp, P1, P2, n);
       MVM_CHECK_LAUNCH();
     }

@@ -69,6 +69,12 @@ def _round_up(x, m):
     return (x + m - 1) // m * m
 
 
+def image_wh(data, i):
+    """(width, height) of data['image{i}'], the size normalize_keypoints divides by (superglue.py:65-72)."""
+    h, w = data['image' + str(i)].shape[-2:]
+    return w, h
+
+
 class MatcherEngine:
     """Shape-keyed workspaces + the C-ABI call.  Shared by MultiViewMatcher and SuperGlue."""
 
@@ -84,11 +90,13 @@ class MatcherEngine:
             self._ws[key] = buf
         return buf
 
-    def run(self, packed, views, img_wh, pair_ids, sinkhorn_iters, match_threshold):
-        """views: list (per view slot) of (kpts [B,n,2], scores [B,n], desc [B,256,n]) CUDA tensors.
+    def run(self, packed, views, view_wh, pair_ids, sinkhorn_iters, match_threshold):
+        """views: list (per view slot) of (kpts [B,n,2], scores [B,n], desc [B,256,n]) CUDA tensors; view_wh: list (per
+        view slot) of the (width, height) its keypoints are normalised by.
         Returns {pair: dict of output tensors} following the reference's shapes/dtypes."""
         lib = _lib.lib()
         T = len(views)
+        assert len(view_wh) == T
         B = views[0][0].shape[0]
         dev = views[0][0].device
         counts = [int(v[0].shape[1]) for v in views]
@@ -130,11 +138,20 @@ class MatcherEngine:
         nbytes = lib.mvm_matcher_workspace_bytes(B, T, n_pad, n_pairs, int(packed.has_conf))
         ws = self.workspace(nbytes, dev)
         cnt = (C.c_int * T)(*counts)
+        wh = [(float(w), float(h)) for w, h in view_wh]
         with torch.cuda.device(dev):
-            rc = lib.mvm_matcher_forward(
-                C.byref(packed.struct), B, T, n_pad, cnt, _lib.ptr(kp), _lib.ptr(sc), _lib.ptr(de),
-                float(img_wh[0]), float(img_wh[1]), int(sinkhorn_iters), float(match_threshold),
-                pairs, n_pairs, _lib.ptr(ws), nbytes, _lib.stream_ptr())
+            if len(set(wh)) == 1:
+                # one image size for every view: the plain entry point (the same arithmetic, bit for bit)
+                rc = lib.mvm_matcher_forward(
+                    C.byref(packed.struct), B, T, n_pad, cnt, _lib.ptr(kp), _lib.ptr(sc), _lib.ptr(de),
+                    wh[0][0], wh[0][1], int(sinkhorn_iters), float(match_threshold),
+                    pairs, n_pairs, _lib.ptr(ws), nbytes, _lib.stream_ptr())
+            else:
+                table = (C.c_float * (2 * T))(*[x for pair in wh for x in pair])
+                rc = lib.mvm_matcher_forward_views(
+                    C.byref(packed.struct), B, T, n_pad, cnt, _lib.ptr(kp), _lib.ptr(sc), _lib.ptr(de),
+                    table, int(sinkhorn_iters), float(match_threshold),
+                    pairs, n_pairs, _lib.ptr(ws), nbytes, None, _lib.stream_ptr())
         _lib.check(rc, 'mvm_matcher_forward')
         # device-resident state the pose stage continues from (no host round trip)
         self.last = {'kpts': kp, 'counts': counts, 'n_pad': n_pad, 'pairs': pairs, 'pair_ids': list(pair_ids),
@@ -241,11 +258,10 @@ class MultiViewMatcher(nn.Module):
                         if k0.shape[1] == 0 or k1.shape[1] == 0:
                             self._empty_pair(result, k0, k1, id0, id1)
                             continue
-                        h, w = data['image' + str(id0)].shape[-2:]
-                        h1, w1 = data['image' + str(id1)].shape[-2:]
-                        assert (h, w) == (h1, w1), 'pair with different image sizes: not supported'
+                        # each view normalised by its own image (multi_view_matcher.py:165-166)
                         outs = self._engine.run(packed, [self._view(data, id0), self._view(data, id1)],
-                                                (w, h), [(0, 1)], iters, self.match_threshold)
+                                                [image_wh(data, id0), image_wh(data, id1)], [(0, 1)], iters,
+                                                self.match_threshold)
                         self._engine.last['view_ids'] = [id0, id1]
                         self._publish(result, outs, {0: id0, 1: id1})
                 return result
@@ -257,10 +273,10 @@ class MultiViewMatcher(nn.Module):
                         self._empty_pair(result, data['keypoints' + str(id0)],
                                          data['keypoints' + str(id1)], id0, id1)
             if len(with_kpts) >= 2:
-                h, w = data['image0'].shape[-2:]   # "assume all images have the same size" (:264)
+                wh = image_wh(data, 0)   # "assume all images have the same size" (:264)
                 slot = {i: s for s, i in enumerate(with_kpts)}
                 pair_ids = [(slot[i0], slot[i1]) for i1 in with_kpts for i0 in with_kpts if i0 < i1]
-                outs = self._engine.run(packed, [self._view(data, i) for i in with_kpts], (w, h),
+                outs = self._engine.run(packed, [self._view(data, i) for i in with_kpts], [wh] * len(with_kpts),
                                         pair_ids, iters, self.match_threshold)
                 self._engine.last['view_ids'] = list(with_kpts)     # slot -> view id of the caller's data dict
                 self._publish(result, outs, {s: i for i, s in slot.items()})

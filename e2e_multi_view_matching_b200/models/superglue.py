@@ -7,7 +7,7 @@ from torch import nn
 
 from .. import _lib
 from ..packing import PackedMatcher
-from .multi_view_matcher import KeypointEncoder, AttentionalGNN, MatcherEngine
+from .multi_view_matcher import KeypointEncoder, AttentionalGNN, MatcherEngine, image_wh
 
 
 class SuperGlue(nn.Module):
@@ -59,14 +59,13 @@ class SuperGlue(nn.Module):
             }
         if kpts0.device.type != 'cuda':
             raise _lib.MvmError('SuperGlue needs CUDA tensors (no CPU fallback)')
-        h, w = data['image0'].shape[-2:]
-        assert tuple(data['image1'].shape[-2:]) == (h, w), 'different image sizes: not supported'
         packed = self._pack(kpts0.device)
         views = [(data['keypoints%d' % i].float(), data['scores%d' % i].float(),
                   data['descriptors%d' % i].float()) for i in (0, 1)]
         with torch.no_grad():
-            o = self._engine.run(packed, views, (w, h), [(0, 1)], self.config['sinkhorn_iterations'],
-                                 self.config['match_threshold'])[(0, 1)]
+            # each view normalised by its own image (superglue.py:245-246)
+            o = self._engine.run(packed, views, [image_wh(data, 0), image_wh(data, 1)], [(0, 1)],
+                                 self.config['sinkhorn_iterations'], self.config['match_threshold'])[(0, 1)]
         return {
             'matches0': o['matches_a'],
             'matches1': o['matches_b'],

@@ -93,7 +93,9 @@ class SuperPoint(nn.Module):
         return self._packed
 
     def dense(self, images):
-        """images [B,1,H,W] -> (scores after NMS [B,H,W], dense descriptors [B,H/8,W/8,256])."""
+        """images [B,1,H,W], any H, W >= 16 -> (scores after NMS [B,8*(H//8),8*(W//8)], dense descriptors
+        [B,H//8,W//8,256]): the three 2x2 pools floor odd sizes, so the last H % 8 rows and W % 8 columns get no score,
+        as in the reference."""
         lib = _lib.lib()
         if images.device.type != 'cuda':
             raise _lib.MvmError('SuperPoint needs CUDA tensors (no CPU fallback)')
@@ -102,7 +104,7 @@ class SuperPoint(nn.Module):
         dev = images.device
         W, _ = self._pack(dev)
         img = images.float().reshape(B, H, Wd).contiguous()
-        scores = torch.empty(B, H, Wd, dtype=torch.float32, device=dev)
+        scores = torch.empty(B, H // 8 * 8, Wd // 8 * 8, dtype=torch.float32, device=dev)
         dense = torch.empty(B, H // 8, Wd // 8, 256, dtype=torch.float32, device=dev)
         nbytes = lib.mvm_superpoint_workspace_bytes(B, H, Wd)
         if self._ws is None or self._ws.numel() < nbytes or self._ws.device != dev:
@@ -115,7 +117,8 @@ class SuperPoint(nn.Module):
 
     def forward(self, data):
         """Compute keypoints, scores, descriptors for the images (superpoint.py:143-229): data['image'] is an iterable of
-        [B,1,H,W] batches; returns lists over all images."""
+        [B,1,H,W] batches (batches may differ in size, as with merge=False in eval_pairs.py); returns lists over all
+        images."""
         lib = _lib.lib()
         all_keypoints, all_scores, all_descriptors = [], [], []
         with torch.no_grad():

@@ -19,6 +19,7 @@ import torch
 
 from .. import _lib
 from .. import ops
+from .multi_view_matcher import image_wh
 
 
 def _round_up(x, m):
@@ -84,17 +85,21 @@ def _forward(model, data, view_ids=None, save=False, debug=None):
     assert N > 0 and all(v[0].shape[:2] == (B, N) for v in views), 'training uses a fixed number of keypoints per view'
     n_pad = max(64, _round_up(N, 64))
     rows = B * T * n_pad
-    h_img, w_img = data['image0'].shape[-2:]
     S = _Saved() if save else None
     # ---- gather the views (one launch) -> point-major rows, slot = b * T + t
     with _lib.device_ctx(dev):
         kp, sc, de = ops.pack_views([tuple(x.detach().float().contiguous() for x in v) for v in views], n_pad)
     x_desc = de.permute(0, 1, 3, 2).reshape(rows, 256).contiguous()
-    # ---- normalize_keypoints (superglue.py:65-72) + KeypointEncoder (multi_view_matcher.py:24-37)
-    center = torch.tensor([w_img / 2.0, h_img / 2.0], dtype=torch.float32, device=dev)
-    scaling = 0.7 * float(max(w_img, h_img))
+    # ---- normalize_keypoints (superglue.py:65-72) + KeypointEncoder (multi_view_matcher.py:24-37): the multi-frame
+    # branch normalises every view by image0 ("assume all images have the same size", :264), the pairwise one each view
+    # by its own image (:165-166)
+    wh = [image_wh(data, 0)] * T if view_ids is None else [image_wh(data, i) for i in ids]
     inp = torch.zeros(rows, 16, dtype=torch.float32, device=dev)
-    inp[:, 0:2] = ((kp - center) / scaling).reshape(rows, 2)
+    inp_slots = inp.view(B, T, n_pad, 16)
+    for t, (w_img, h_img) in enumerate(wh):
+        center = torch.tensor([w_img / 2.0, h_img / 2.0], dtype=torch.float32, device=dev)
+        scaling = 0.7 * float(max(w_img, h_img))
+        inp_slots[:, t, :, 0:2] = (kp[:, t] - center) / scaling
     inp[:, 2] = sc.reshape(rows)
     enc = model.kenc.encoder
     h = inp

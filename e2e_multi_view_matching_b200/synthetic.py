@@ -163,16 +163,20 @@ def make_correlated_view_inputs(seed, n_views, n_kpts, batch=1, width=640, heigh
 
 
 def make_scene_tuple_inputs(seed, n_views=5, n_kpts=1024, batch=1, width=640, height=480, f=577.87,
-                            desc_dim=256, desc_noise=0.25, noise_px=1.0):
+                            desc_dim=256, desc_noise=0.25, noise_px=1.0, sizes=None):
     """Geometrically consistent synthetic tuples for the end-to-end bench: 3-D landmarks (depth
     2..6 m) seen by `n_views` cameras (view 0 identity, others rotated <= 12 deg, baseline <= 0.6 m),
     pixel keypoints with `noise_px` noise, descriptors = landmark descriptor + noise (unit norm),
-    scores U(0,1), K = [[f,0,(w-1)/2],[0,f,(h-1)/2],[0,0,1]].  Returns the matcher `data` dict
-    (numpy) with intr{i} [B,3,3], pose{i} [B,4,4] (cam->world ground truth, the reference's convention) and
-    extr{i} (its inverse, world->cam)."""
+    scores U(0,1), K = [[f,0,(w-1)/2],[0,f,(h-1)/2],[0,0,1]].  `sizes`: optional list of one (width, height)
+    per view (e.g. a portrait and a landscape image of a pair); each view then has its own K and image{i} shape, and
+    the landmarks are the ones that project inside every view's image.  Default: (width, height) for every view.
+    Returns the matcher `data` dict (numpy) with intr{i} [B,3,3], pose{i} [B,4,4] (cam->world ground truth, the
+    reference's convention) and extr{i} (its inverse, world->cam)."""
     rng = np.random.default_rng(seed)
-    K = np.array([[f, 0, (width - 1) / 2], [0, f, (height - 1) / 2], [0, 0, 1.0]])
-    Kinv = np.linalg.inv(K)
+    sizes = [(width, height)] * n_views if sizes is None else [tuple(s) for s in sizes]
+    assert len(sizes) == n_views
+    Ks = [np.array([[f, 0, (w - 1) / 2], [0, f, (h - 1) / 2], [0, 0, 1.0]]) for w, h in sizes]
+    Kinv = np.linalg.inv(Ks[0])
     out = {}
 
     def rod(w):
@@ -197,17 +201,17 @@ def make_scene_tuple_inputs(seed, n_views=5, n_kpts=1024, batch=1, width=640, he
         while land.shape[0] < n_land:
             m = 4 * n_land
             z = rng.uniform(2, 6, m)
-            uv = rng.uniform([30, 30], [width - 30, height - 30], size=(m, 2))
+            uv = rng.uniform([30, 30], [sizes[0][0] - 30, sizes[0][1] - 30], size=(m, 2))
             X = (Kinv @ np.concatenate([uv, np.ones((m, 1))], 1).T).T * z[:, None]
             ok = np.ones(m, bool)
-            for T in poses:
+            for T, K, (w, h) in zip(poses, Ks, sizes):
                 q = X @ T[:3, :3].T + T[:3, 3]
                 px = (q @ K.T)[:, :2] / q[:, 2:3]
-                ok &= (q[:, 2] > 0.5) & (px[:, 0] >= 0) & (px[:, 0] < width) & (px[:, 1] >= 0) & (px[:, 1] < height)
+                ok &= (q[:, 2] > 0.5) & (px[:, 0] >= 0) & (px[:, 0] < w) & (px[:, 1] >= 0) & (px[:, 1] < h)
             land = np.concatenate([land, X[ok]], 0)
         land = land[:n_land]
         land_desc = rng.standard_normal((n_land, desc_dim))
-        for i, T in enumerate(poses):
+        for i, (T, K) in enumerate(zip(poses, Ks)):
             sel = rng.permutation(n_land)[:n_kpts]
             q = land[sel] @ T[:3, :3].T + T[:3, 3]
             px = (q @ K.T)[:, :2] / q[:, 2:3] + noise_px * rng.standard_normal((n_kpts, 2))
@@ -222,8 +226,8 @@ def make_scene_tuple_inputs(seed, n_views=5, n_kpts=1024, batch=1, width=640, he
             out.setdefault('landmark%d' % i, []).append(sel.astype(np.int64))
     for k in list(out.keys()):
         out[k] = np.stack(out[k], 0)
-    for i in range(n_views):
-        out['image%d' % i] = np.zeros((batch, 1, height, width), np.float32)
+    for i, (w, h) in enumerate(sizes):
+        out['image%d' % i] = np.zeros((batch, 1, h, w), np.float32)
     out['ids'] = list(range(n_views))
     return out
 

@@ -103,7 +103,8 @@ size_t mvm_matcher_workspace_bytes(int batch, int n_views, int n_pad, int n_pair
  *   kpts      [batch*n_views, n_pad, 2]  pixel x,y        (device)
  *   kscores   [batch*n_views, n_pad]                       (device)
  *   desc      [batch*n_views, 256, n_pad] channel-first    (device)
- *   img_w/h   image size used by normalize_keypoints (superglue.py:65-72)
+ *   img_w/h   image size used by normalize_keypoints (superglue.py:65-72), the same for every view
+ *             (mvm_matcher_forward_views takes one size per view)
  *   pairs     host array of n_pairs descriptors with device output pointers
  *   match_threshold  0 for MultiViewMatcher (:297), 0.2 for SuperGlue (superglue.py:275) */
 int mvm_matcher_forward(const mvm_matcher_weights* w, int batch, int n_views, int n_pad,
@@ -134,6 +135,18 @@ int mvm_matcher_forward_ex(const mvm_matcher_weights* w, int batch, int n_views,
                            float match_threshold, const mvm_pair_io* pairs, int n_pairs,
                            void* workspace, size_t workspace_bytes, const mvm_matcher_options* opt /* NULL = defaults */,
                            void* stream);
+
+/* mvm_matcher_forward_ex with one image size per view slot, for pairs whose images differ in size (the pairwise
+ * matcher normalises each view by its own image, multi_view_matcher.py:165-166, superglue.py:245-246):
+ *   view_wh   HOST float[n_views][2]: (width, height) of view slot t, shared by the batch; keypoint k of slot t is
+ *             normalised as (k - wh/2) / (0.7 * max(w, h)) in fp32.
+ * mvm_matcher_forward and _ex call this with every entry equal to (img_w, img_h); the results are bitwise the same. */
+int mvm_matcher_forward_views(const mvm_matcher_weights* w, int batch, int n_views, int n_pad,
+                              const int* counts, const float* kpts, const float* kscores,
+                              const float* desc, const float* view_wh, int sinkhorn_iters,
+                              float match_threshold, const mvm_pair_io* pairs, int n_pairs,
+                              void* workspace, size_t workspace_bytes, const mvm_matcher_options* opt /* NULL = defaults */,
+                              void* stream);
 
 /* ---- individual stages (exported for stage-parity tests and for callers that only need
  * one stage; same semantics as the fused forward) -------------------------------------- */
@@ -376,9 +389,11 @@ typedef struct mvm_superpoint_weights {
 
 size_t mvm_superpoint_workspace_bytes(int batch, int height, int width);
 
-/* Dense part of SuperPoint.forward (:150-170, :213-216): image [batch, height, width] fp32 (grayscale in [0,1]; height,
- * width multiples of 8) -> scores_nms [batch, height, width] (softmax keypoint scores after simple_nms, 0 where
- * suppressed) and dense_desc [batch, height/8, width/8, 256] (L2-normalised, channels last). */
+/* Dense part of SuperPoint.forward (:150-170, :213-216): image [batch, height, width] fp32 (grayscale in [0,1]; any
+ * height, width >= 16) -> scores_nms [batch, 8*floor(height/8), 8*floor(width/8)] (softmax keypoint scores after
+ * simple_nms, 0 where suppressed) and dense_desc [batch, floor(height/8), floor(width/8), 256] (L2-normalised, channels
+ * last).  The three 2x2 pools floor odd sizes like nn.MaxPool2d, so the last height % 8 rows and width % 8 columns of the
+ * image have no score, as in the reference (:169-172). */
 int mvm_superpoint_dense(const mvm_superpoint_weights* w, const float* image, int batch, int height, int width,
                          int nms_radius, float* scores_nms, float* dense_desc, void* workspace, size_t workspace_bytes,
                          void* stream);
