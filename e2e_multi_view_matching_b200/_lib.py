@@ -137,6 +137,9 @@ def lib():
     L.mvm_linear_tc_h16.restype = C.c_int
     L.mvm_linear_tc_h16.argtypes = [_fp, C.c_int, _fp, C.c_int, C.c_int, _fp, _fp, C.c_float, C.c_int, _fp, _fp, C.c_int,
                                     _fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, _fp]
+    L.mvm_qkv_projection.restype = C.c_int
+    L.mvm_qkv_projection.argtypes = [_fp, _fp, _fp, _fp, _fp, C.c_float, _fp, _fp, C.c_int, C.c_int, C.c_int,
+                                     _fp, _fp, _fp, _fp, _fp]
     L.mvm_linear_tc.restype = C.c_int
     L.mvm_linear_tc.argtypes = [_fp, C.c_int, _fp, C.c_int, C.c_int, _fp, C.c_int, _fp, _fp, C.c_int,
                                 _fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _fp]

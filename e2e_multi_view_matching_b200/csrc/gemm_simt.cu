@@ -146,10 +146,9 @@ int launch_score_gemm_simt(const float* mdesc, int n_pad, const PairTable& tab, 
 }
 
 int launch_gemm_simt(const GemmDesc& g, cudaStream_t stream) {
+  static_assert(BK == 16, "gemm_desc_valid(GEMM_SIMT) states K in k-blocks of 16");
+  MVM_REQUIRE(gemm_desc_valid(g, GEMM_SIMT));
   MvmProfScope prof__(MVM_TAG_GEMM, stream);
-  MVM_REQUIRE(g.K % BK == 0 && g.K1 % BK == 0);
-  MVM_REQUIRE(g.lda % 4 == 0 && g.ldw % 4 == 0 && (g.A2 == nullptr || g.lda2 % 4 == 0));
-  MVM_REQUIRE(g.M > 0 && g.N > 0 && g.batch > 0);
   dim3 grid(mvm_div_up(g.N, BN), mvm_div_up(g.M, BM), g.batch);
   gemm_simt_kernel<<<grid, 256, 0, stream>>>(g);
   MVM_CHECK_LAUNCH();

@@ -18,7 +18,7 @@
 //                    wgmma of k-block kt are issued before the A fragments of kt + 1 are split, so the split runs under
 //                    them (two fragment sets in registers, raised to 232 per thread by setmaxnreg), and the epilogue
 //                    loads its bias / residual operands in batches
-//   warp 8           TMA producer (with BN = 128 warps 8-11, the producer warpgroup, 40 registers): one lane issues the
+//   warps 8-11       the producer warpgroup (40 registers): one lane of warp 8 issues the
 //                    TMA loads of A [128 x BK] (fp32) and the W planes [BN x 128 B] into a STAGES-deep ring
 // The tile schedule is static: with `persistent` one CTA per SM walks the tiles (the producer fills the ring for the
 // next tile under the epilogue of the current one), otherwise one tile per CTA.  Both issue the same instructions per
@@ -36,10 +36,11 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int PRODUCER_WARP = 8;
-// 128-column tiles: 384 threads (warps 8-11 are the producer warpgroup) and setmaxnreg 2 x 232 + 40 = the 504 per-thread
-// registers of one SM sub-partition (one warp of each warpgroup), for the pipelined mainloop.  256-column tiles: 288
-// threads (one producer warp) and the in-order mainloop.
-template <int BN> constexpr int nthreads() { return BN == 128 ? 384 : 288; }
+// 384 threads (warps 8-11 are the producer warpgroup) and setmaxnreg 2 x 232 + 40 = the 504 per-thread registers of one
+// SM sub-partition (one warp of each warpgroup): the second fragment set of the pipelined mainloop (128-column tiles), or
+// the 128 accumulators of the in-order one (256-column tiles).  ptxas budgets a wgmma kernel by whole warpgroups, so
+// 288 threads would cap every thread at 168 registers, and the 256-column instances spilled under that cap.
+constexpr int NTHREADS = 384;
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 enum { W_RAW = 0, W_TF32 = 1, W_F16 = 2 };
 
@@ -106,7 +107,7 @@ __device__ __forceinline__ void fence_afrag(uint32_t (&a)[4][4]) {
 }
 
 template <int BN, int NPASS, int WM, bool SCORE>
-__global__ void __launch_bounds__(nthreads<BN>(), 1)
+__global__ void __launch_bounds__(NTHREADS, 1)
 gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                const __grid_constant__ CUtensorMap tmWhi, const __grid_constant__ CUtensorMap tmWlo,
                const __grid_constant__ GArgs g, const __grid_constant__ ScoreTab st) {
@@ -150,7 +151,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   if (warp >= PRODUCER_WARP) {
     // ================================ TMA producer ================================
-    if (PIPE) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
     if (warp == PRODUCER_WARP && lane == 0) {
       tc::prefetch_tmap(&tmA); tc::prefetch_tmap(&tmA2); tc::prefetch_tmap(&tmWhi); tc::prefetch_tmap(&tmWlo);
       uint32_t it = 0;
@@ -178,7 +179,7 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 
   // ================================ consumers ================================
-  if (PIPE) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
   const int wg = warp >> 2, wq = warp & 3;
   const int gr = lane >> 2, tq = lane & 3;
   const int row0 = wg * 64 + wq * 16 + gr;                     // tile rows of this thread: row0, row0 + 8
@@ -430,7 +431,7 @@ int launch_wg(const CUtensorMap* tA, const CUtensorMap* tA2, const CUtensorMap* 
   cudaFuncSetAttribute(gemm_wg_kernel<BN, NPASS, WM, SCORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES);
   const int n_sm = mvm_dev_info().n_sm;
   const int grid = (persistent && n_tiles > n_sm) ? n_sm : (int)n_tiles;
-  gemm_wg_kernel<BN, NPASS, WM, SCORE><<<grid, nthreads<BN>(), C_::SMEM_BYTES, stream>>>(*tA, *tA2, *tWhi, *tWlo, g, st);
+  gemm_wg_kernel<BN, NPASS, WM, SCORE><<<grid, NTHREADS, C_::SMEM_BYTES, stream>>>(*tA, *tA2, *tWhi, *tWlo, g, st);
   MVM_CHECK_LAUNCH();
   return MVM_OK;
 }
@@ -571,8 +572,8 @@ extern "C" void mvm_debug_set_gemm_tile(int bn) { g_gemm_bn = bn == 256 ? 256 : 
 int g_gemm_persist = 1;   // 1: the persistent schedule with pre-split W planes serves the 3xTF32 path (default)
 extern "C" void mvm_debug_set_gemm_kernel(int persistent) { g_gemm_persist = persistent ? 1 : 0; }
 
-// GEMM on the tensor cores.  Requirements: K, K1 multiples of 32, N multiple of 128, 16-byte aligned
-// rows (lda/ldw/ldc/ldr multiples of 4).  n_pass: 3 = fp32-faithful 3xTF32, 1 = single-pass TF32.
+// GEMM on the tensor cores.  Requirements: gemm_desc_valid(d, GEMM_TC_TF32) (kernels.cuh).  n_pass: 3 = fp32-faithful
+// 3xTF32, 1 = single-pass TF32.
 int mvm_default_gemm_tile() { return g_gemm_bn; }
 int mvm_default_gemm_persistent() { return g_gemm_persist; }
 
@@ -580,9 +581,9 @@ int launch_gemm_tc(const GemmDesc& d, int n_pass, float* VT, int vt_col0, int n_
                    float* KLO, float* VTLO, int gemm_tile, int gemm_persist) {
   if (gemm_tile < 0) gemm_tile = g_gemm_bn;            // stage-level callers: the process defaults
   if (gemm_persist < 0) gemm_persist = g_gemm_persist;
-  MVM_REQUIRE(d.batch == 1 && d.K % 32 == 0 && d.K1 % 32 == 0 && d.N % 128 == 0);
-  MVM_REQUIRE(d.lda % 4 == 0 && d.ldw % 4 == 0 && d.ldc % 4 == 0 && (d.R == nullptr || d.ldr % 4 == 0));
-  MVM_REQUIRE(d.A2 == nullptr || d.lda2 % 4 == 0);
+  MVM_REQUIRE(gemm_desc_valid(d, GEMM_TC_TF32));
+  MVM_REQUIRE(d.W || (n_pass == 3 && d.Whi && d.Wlo));
+  MVM_REQUIRE(mvm_aligned(KLO, 8));
   MvmProfScope prof__(MVM_TAG_GEMM, stream);
   if (gemm_persist && n_pass == 3 && d.Whi && d.Wlo) return launch_gemm_tc_persist(d, VT, vt_col0, n_pad, KLO, VTLO, stream);
   if (gemm_tile == 256 && d.N % 256 == 0) {
@@ -595,7 +596,8 @@ int launch_gemm_tc(const GemmDesc& d, int n_pass, float* VT, int vt_col0, int n_
 }
 
 // Persistent schedule, 128-column tiles, W given as its tf32 planes or (fp16x3) as half-precision planes of
-// wscale * W.  Requirements as launch_gemm_tc; the fp16 planes are used when given and K, K1 are multiples of 64.
+// wscale * W.  Requirements: gemm_desc_valid(d, GEMM_TC_F16) for the fp16 planes, which are used when given and K, K1
+// are multiples of 64; otherwise gemm_desc_valid(d, GEMM_TC_TF32) and both tf32 planes.
 int launch_gemm_tc_persist(const GemmDesc& d, float* VT, int vt_col0, int n_pad, float* KLO, float* VTLO,
                            cudaStream_t stream, const HalfPlanes* hp, int ksplit, float* slabs) {
   // split-K: partial products of the K slices go to slabs [ksplit, M, N] (M a multiple of the tile height), summed by
@@ -603,6 +605,9 @@ int launch_gemm_tc_persist(const GemmDesc& d, float* VT, int vt_col0, int n_pad,
   MVM_REQUIRE(ksplit >= 1 && (ksplit == 1 || (slabs && d.M % BM == 0 && d.K % (32 * ksplit) == 0 && !d.Whi16 && !d.bias && !d.R && !d.A2 &&
                                                !d.relu && !VT && !KLO && !hp)));
   const bool f16 = d.Whi16 != nullptr && d.Wlo16 != nullptr && d.K % 64 == 0 && d.K1 % 64 == 0 && d.wscale > 0.f;
+  MVM_REQUIRE(f16 ? gemm_desc_valid(d, GEMM_TC_F16) : gemm_desc_valid(d, GEMM_TC_TF32) && d.Whi && d.Wlo);
+  MVM_REQUIRE(mvm_aligned(KLO, 8) && mvm_aligned(slabs, 16));
+  MVM_REQUIRE(!hp || (mvm_aligned(hp->kh, 4) && mvm_aligned(hp->kl, 4) && mvm_aligned(hp->vh, 4) && mvm_aligned(hp->vl, 4)));
   const CUtensorMap* tA = mvm_get_tmap_2d(d.A, d.M, d.K1, d.lda, BM);
   const CUtensorMap* tA2 = d.A2 ? mvm_get_tmap_2d(d.A2, d.M, d.K - d.K1, d.lda2, BM) : tA;
   GArgs g = make_args(d, VT, vt_col0, n_pad, KLO, VTLO, 128);
@@ -624,7 +629,7 @@ int launch_gemm_tc_persist(const GemmDesc& d, float* VT, int vt_col0, int n_pad,
 }
 
 int launch_splitk_reduce(const float* slabs, float* C, int M, int N, int ldc, int ksplit, cudaStream_t stream) {
-  MVM_REQUIRE(N % 4 == 0 && ldc % 4 == 0);
+  MVM_REQUIRE(N % 4 == 0 && ldc % 4 == 0 && mvm_aligned(slabs, 16) && mvm_aligned(C, 16));
   const long long n = (long long)M * (N / 4);
   splitk_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(slabs), C, M, N / 4, ldc, ksplit);
   MVM_CHECK_LAUNCH();

@@ -29,6 +29,37 @@ int launch_kenc_front(const float* kpts, const float* kscores, const float* cons
 int launch_transpose_cn(const float* in, float* out, int n_views_total, int C, int n_pad,
                         cudaStream_t stream);
 
+// What every GEMM launch needs of its descriptor, checked on the host before any CUDA call (a bad call returns
+// MVM_ERR_INVALID instead of failing a tensor-map encode or faulting in the kernel).  `ops` names the kernel family:
+//   GEMM_SIMT     fp32 CUDA cores: float4 loads of A, A2 and W (16-byte aligned, lda / lda2 / ldw multiples of 4),
+//                 K and K1 multiples of 16
+//   GEMM_TC_TF32  tensor cores with tf32 operands: TMA boxes of A, A2 and the W planes (16-byte aligned base, row
+//                 pitch a multiple of 16 bytes), K and K1 multiples of 32, N of 128, float2 epilogue stores and residual
+//                 loads (C and R 8-byte aligned, ldc / ldr multiples of 4)
+//   GEMM_TC_F16   as GEMM_TC_TF32 with W given as fp16 planes (ldw a multiple of 8), K and K1 multiples of 64
+// Always: M >= 1, K >= one k-block, and K1 == K without A2 (0 < K1 < K with it).
+enum { GEMM_SIMT = 0, GEMM_TC_TF32 = 1, GEMM_TC_F16 = 2 };
+inline bool mvm_aligned(const void* p, unsigned bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+inline bool gemm_desc_valid(const GemmDesc& d, int ops) {
+  const bool tc = ops != GEMM_SIMT;
+  const int bk = ops == GEMM_SIMT ? 16 : ops == GEMM_TC_TF32 ? 32 : 64;
+  if (!d.A || !d.C || d.M < 1 || d.N < 1 || d.K < bk || d.K % bk != 0 || d.K1 % bk != 0) return false;
+  if (d.A2 ? (d.K1 <= 0 || d.K1 >= d.K) : d.K1 != d.K) return false;
+  if (!mvm_aligned(d.A, 16) || d.lda % 4 != 0) return false;
+  if (d.A2 && (!mvm_aligned(d.A2, 16) || d.lda2 % 4 != 0)) return false;
+  // W operand: raw fp32 (SIMT, the raw-W tensor-core kernels) or its pre-split tf32 / fp16 planes
+  if (ops == GEMM_SIMT && !d.W) return false;
+  if (ops == GEMM_TC_TF32 && !d.W && !(d.Whi && d.Wlo)) return false;
+  if (ops == GEMM_TC_F16 && !(d.Whi16 && d.Wlo16 && d.wscale > 0.f)) return false;
+  const void* w[5] = {d.W, d.Whi, d.Wlo, d.Whi16, d.Wlo16};
+  for (const void* p : w)
+    if (p && !mvm_aligned(p, 16)) return false;
+  if (d.ldw % (ops == GEMM_TC_F16 ? 8 : 4) != 0) return false;
+  if (!tc) return d.batch >= 1;
+  return d.batch == 1 && d.N % 128 == 0 && mvm_aligned(d.C, 8) && d.ldc % 4 == 0 &&
+         (!d.R || (mvm_aligned(d.R, 8) && d.ldr % 4 == 0));
+}
+
 // tensor-core GEMM (gemm_tc.cu): n_pass 3 = fp32-faithful 3xTF32, 1 = single-pass TF32
 // gemm_tile (128 / 256) and gemm_persist (0 / 1) select the kernel; -1 = the process defaults
 int launch_gemm_tc(const GemmDesc& d, int n_pass, float* VT, int vt_col0, int n_pad, cudaStream_t stream,

@@ -102,6 +102,21 @@ int run_gemm(const Ctx& cx, const GemmDesc& g_in, cudaStream_t s) {
   return launch_gemm_simt(g, s);
 }
 
+// The QKV projection of a GNN layer, x [rows, 256] -> [rows, 768], with its W planes already in the descriptor (qkv_desc
+// + the caller's planes).  K and V leave as the operand planes of the attention that follows: fp16 hi / lo planes (hp,
+// the fp16x3 attention), or V^T [rows / n_pad, 256, n_pad] (VT) and, in 3xTF32, the tf32 remainders of K and V^T.
+GemmDesc qkv_desc(const float* X, const float* W, const float* bias, float* qkv, int rows) {
+  return make_gemm(X, 256, W, 256, bias, qkv, 768, rows, 768, 0);
+}
+int run_qkv(const GemmDesc& gq, int n_pass, int n_pad, const HalfPlanes* hp, float* VT, float* KLO, float* VTLO,
+            int gemm_tile, int gemm_persist, cudaStream_t s) {
+  if (hp) {
+    MvmProfScope prof__(MVM_TAG_GEMM, s);      // (launch_gemm_tc opens the scope on the other path)
+    return launch_gemm_tc_persist(gq, nullptr, 512, n_pad, nullptr, nullptr, s, hp);
+  }
+  return launch_gemm_tc(gq, n_pass, VT, 512, n_pad, s, KLO, VTLO, gemm_tile, gemm_persist);
+}
+
 #define MVM_TRY(x)            \
   do {                        \
     int rc__ = (x);           \
@@ -228,21 +243,18 @@ int mvm_matcher_forward_views(const mvm_matcher_weights* w, int batch, int n_vie
       __half* kh = reinterpret_cast<__half*>(ws.KLO);
       __half* vh = reinterpret_cast<__half*>(ws.VTLO);
       HalfPlanes hp = {kh, kh + (size_t)rows * 256, vh, vh + (size_t)rows * 256};
-      GemmDesc gq = make_gemm(ws.X, 256, L.w_qkv, 256, L.b_qkv, ws.QKV, 768, rows, 768, 0);
+      GemmDesc gq = qkv_desc(ws.X, L.w_qkv, L.b_qkv, ws.QKV, rows);
       set_planes(cx, gq);
-      {
-        MvmProfScope prof__(MVM_TAG_GEMM, s);      // (launch_gemm_tc opens the scope on the other paths)
-        MVM_TRY(launch_gemm_tc_persist(gq, nullptr, 512, n_pad, nullptr, nullptr, s, &hp));
-      }
+      MVM_TRY(run_qkv(gq, cx.math_mode, n_pad, &hp, nullptr, nullptr, nullptr, cx.gemm_tile, cx.gemm_persist, s));
       MVM_TRY(launch_attention_h3(ws.QKV, (const __half*)hp.kh, (const __half*)hp.kl, (const __half*)hp.vh,
                                   (const __half*)hp.vl, ws.MSG, batch, n_pad, segs, L.is_cross, s));
     } else if (cx.math_mode != 0) {
       // tensor-core path: the QKV GEMM epilogue also writes V^T [view, 256, n_pad] for the P.V product
       float* klo = cx.math_mode == 3 ? ws.KLO : nullptr;
       float* vtlo = cx.math_mode == 3 ? ws.VTLO : nullptr;
-      GemmDesc gq = make_gemm(ws.X, 256, L.w_qkv, 256, L.b_qkv, ws.QKV, 768, rows, 768, 0);
+      GemmDesc gq = qkv_desc(ws.X, L.w_qkv, L.b_qkv, ws.QKV, rows);
       if (cx.math_mode == 3 && cx.lo_off != 0) { gq.Whi = gq.W + cx.hi_off; gq.Wlo = gq.W + cx.lo_off; }
-      MVM_TRY(launch_gemm_tc(gq, cx.math_mode, ws.VT, 512, n_pad, s, klo, vtlo, cx.gemm_tile, cx.gemm_persist));
+      MVM_TRY(run_qkv(gq, cx.math_mode, n_pad, nullptr, ws.VT, klo, vtlo, cx.gemm_tile, cx.gemm_persist, s));
       MVM_TRY(launch_attention_tc(ws.QKV, ws.VT, ws.MSG, batch, n_pad, segs, L.is_cross, cx.math_mode, s, klo, vtlo));
     } else {
       MVM_TRY(run_gemm(cx, make_gemm(ws.X, 256, L.w_qkv, 256, L.b_qkv, ws.QKV, 768, rows, 768, 0), s));
@@ -372,6 +384,21 @@ int mvm_linear_tc_h16(const float* A, int lda, const float* A2, int lda2, int K1
   if (A2) { g.A2 = A2; g.lda2 = lda2; g.K1 = K1; MVM_REQUIRE(K1 % 64 == 0); }
   if (R) { g.R = R; g.ldr = ldr; }
   return launch_gemm_tc_persist(g, nullptr, 0, 0, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+int mvm_qkv_projection(const float* X, const float* W_hi, const float* W_lo, const void* W16_hi, const void* W16_lo,
+                       float wscale, const float* bias, float* qkv, int rows, int n_pad, int planes16, void* k_hi,
+                       void* k_lo, void* v_hi, void* v_lo, void* stream) {
+  MVM_REQUIRE(X && W_hi && W_lo && qkv && k_lo && v_hi && v_lo && n_pad >= 64 && n_pad % 64 == 0 && rows % n_pad == 0);
+  MVM_REQUIRE(!planes16 || k_hi);
+  MVM_REQUIRE(!W16_hi == !W16_lo && (!W16_hi || wscale > 0.f));
+  // the GNN layer's launch (run_qkv), with the process defaults of the options
+  GemmDesc gq = qkv_desc(X, W_hi, bias, qkv, rows);
+  gq.Whi = W_hi; gq.Wlo = W_lo;
+  if (!planes16) return run_qkv(gq, 3, n_pad, nullptr, (float*)v_hi, (float*)k_lo, (float*)v_lo, -1, -1, (cudaStream_t)stream);
+  if (W16_hi) { gq.Whi16 = W16_hi; gq.Wlo16 = W16_lo; gq.wscale = wscale; }
+  HalfPlanes hp = {k_hi, k_lo, v_hi, v_lo};
+  return run_qkv(gq, 3, n_pad, &hp, nullptr, nullptr, nullptr, -1, -1, (cudaStream_t)stream);
 }
 
 int mvm_attention(const float* qkv, float* out, int batch, int n_views, int n_pad,

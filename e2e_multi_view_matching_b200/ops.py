@@ -12,6 +12,16 @@ def rn_tf32(x):
     return ((x.contiguous().view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32)
 
 
+H16_SCALE = 64.0     # the fp16 planes hold H16_SCALE * W, as packing.py stores them
+
+
+def h16_planes(w):
+    """(hi, lo) fp16 planes of H16_SCALE * w: hi = fp16(s w), lo = fp16(s w - hi)."""
+    ws = w.double() * H16_SCALE
+    w_hi = ws.to(torch.float16)
+    return w_hi.contiguous(), (ws - w_hi.double()).to(torch.float16).contiguous()
+
+
 def linear(a, w, bias=None, a2=None, residual=None, relu=False, alpha=1.0, tc_passes=0, presplit=False):
     """act(alpha * [a|a2] @ w.T + bias) + residual on point-major activations (Conv1d k=1).
     tc_passes: 0 = fp32 CUDA cores, 3 = 3xTF32 on the tensor cores, 1 = single-pass TF32.
@@ -23,11 +33,8 @@ def linear(a, w, bias=None, a2=None, residual=None, relu=False, alpha=1.0, tc_pa
         K = K1 + (a2.shape[1] if a2 is not None else 0)
         N = w.shape[0]
         out = torch.empty(M, N, dtype=torch.float32, device=a.device)
-        scale = 64.0
-        ws = w.double() * scale
-        w_hi = ws.to(torch.float16)
-        w_lo = (ws - w_hi.double()).to(torch.float16).contiguous()
-        w_hi = w_hi.contiguous()
+        scale = H16_SCALE
+        w_hi, w_lo = h16_planes(w)
         rc = lib.mvm_linear_tc_h16(_lib.ptr(a), a.stride(0), _lib.ptr(a2), a2.stride(0) if a2 is not None else 0, K1,
                                    _lib.ptr(w_hi), _lib.ptr(w_lo), scale, w_hi.stride(0), _lib.ptr(bias), _lib.ptr(residual),
                                    residual.stride(0) if residual is not None else 0, _lib.ptr(out), N, M, N, K,
@@ -65,6 +72,33 @@ def linear(a, w, bias=None, a2=None, residual=None, relu=False, alpha=1.0, tc_pa
                         float(alpha), int(relu), _lib.stream_ptr())
     _lib.check(rc, 'mvm_linear')
     return out
+
+
+def qkv_projection(x, w, bias, n_pad, planes='fp16', w16=True, out=None):
+    """The QKV projection of one GNN layer as the matcher launches it (mvm_qkv_projection): x [rows, 256], w [768, 256],
+    bias [768] -> (qkv [rows, 768] with Q in columns 0..255, planes).
+    planes 'fp16': (kh, kl, vh, vl), half [rows, 256], for the fp16x3 attention; W enters as the fp16 planes of
+    H16_SCALE * w (w16) or as its tf32 planes.  planes 'tf32': (klo [rows, 256], vt, vtlo [rows / n_pad, 256, n_pad]),
+    with rn_tf32(K) in columns 256..511 of qkv.  Columns of qkv that go to planes are left as `out` had them."""
+    lib = _lib.lib()
+    rows = x.shape[0]
+    dev = x.device
+    qkv = torch.empty(rows, 768, dtype=torch.float32, device=dev) if out is None else out
+    w_hi = rn_tf32(w)
+    w_lo = rn_tf32(w - w_hi)
+    h_hi, h_lo = h16_planes(w) if (planes == 'fp16' and w16) else (None, None)
+    if planes == 'fp16':
+        p = tuple(torch.empty(rows, 256, dtype=torch.float16, device=dev) for _ in range(4))
+        ptrs = p
+    else:
+        p = (torch.empty(rows, 256, dtype=torch.float32, device=dev),
+             torch.empty(rows // n_pad, 256, n_pad, dtype=torch.float32, device=dev),
+             torch.empty(rows // n_pad, 256, n_pad, dtype=torch.float32, device=dev))
+        ptrs = (None,) + p
+    _lib.check(lib.mvm_qkv_projection(_lib.ptr(x), _lib.ptr(w_hi), _lib.ptr(w_lo), _lib.ptr(h_hi), _lib.ptr(h_lo),
+                                      H16_SCALE, _lib.ptr(bias), _lib.ptr(qkv), rows, n_pad, int(planes == 'fp16'),
+                                      *[_lib.ptr(t) for t in ptrs], _lib.stream_ptr()), 'mvm_qkv_projection')
+    return qkv, p
 
 
 def attention(qkv, batch, n_views, counts, is_cross, tc_passes=0):

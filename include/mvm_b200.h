@@ -158,7 +158,17 @@ int mvm_linear(const float* A, int lda, const float* A2, int lda2, int K1, const
 
 /* Same contract on the tensor cores (tf32 wgmma, TMA-fed, accumulators in registers).
  * n_pass = 3: fp32-faithful 3xTF32 (operands split hi/lo on chip); n_pass = 1: single-pass TF32.
- * Needs N % 128 == 0, K % 32 == 0, K1 % 32 == 0, 16-byte aligned rows. */
+ *
+ * Operand rules of every GEMM entry below and of mvm_linear, checked on the host before any CUDA call; a call that
+ * breaks one returns 1 (invalid argument):
+ *   M >= 1, N >= 1; K and K1 multiples of the k-block and K >= one k-block: 32 here and in the _presplit / _splitk
+ *   entries, 64 in mvm_linear_tc_h16, 16 in mvm_linear; K1 == K without A2, 0 < K1 < K with it;
+ *   A, A2 and W (or its planes) 16-byte aligned, lda, lda2 and ldw multiples of 4 (ldw of 8 for the fp16 planes): the
+ *   tensor-core kernels load them by TMA, mvm_linear by float4;
+ *   tensor cores only: N % 128 == 0, C and R 8-byte aligned with ldc, ldr multiples of 4 (float2 epilogue);
+ *   the _splitk entry: C and ws 16-byte aligned, M and N multiples of 128, K of 32 * ksplit, ksplit >= 2.
+ * Leading dimensions may exceed the logical widths (column slices of wider buffers).  R may be C itself (an in-place
+ * residual, as every GNN layer's mlp.1 does): each output element reads its residual before it is stored. */
 int mvm_linear_tc(const float* A, int lda, const float* A2, int lda2, int K1, const float* W,
                   int ldw, const float* bias, const float* R, int ldr, float* C, int ldc, int M,
                   int N, int K, float alpha, int relu, int n_pass, void* stream);
@@ -177,10 +187,30 @@ int mvm_linear_tc_presplit_splitk(const float* A, int lda, const float* W_hi, co
                                   int M, int N, int K, float alpha, int ksplit, float* ws, void* stream);
 
 /* fp16x3 on the persistent schedule: W16_hi / W16_lo = fp16 planes of wscale * W (hi = fp16(wscale W), lo = fp16(wscale W - hi));
- * K and K1 multiples of 64, N of 128. */
+ * K and K1 multiples of 64, N of 128.
+ * Range of A, which is split on chip the same way (hi = fp16(a), lo = fp16(a - hi)): hi + lo keeps the 22 bits of the
+ * 3xTF32 split only while lo is an fp16 normal, i.e. |a| >= 2^-3; below that lo is exact to 2^-24 absolute, so every
+ * element costs up to 2^-25 |w| of error however small it is, and rows made of small elements lose relative accuracy.
+ * |a| >= 65520 makes hi infinite: the output is inf or NaN where fp32 is finite.  Use the tf32 entries for operands
+ * outside the range given in DESIGN.md section 3. */
 int mvm_linear_tc_h16(const float* A, int lda, const float* A2, int lda2, int K1, const void* W16_hi, const void* W16_lo,
                       float wscale, int ldw, const float* bias, const float* R, int ldr, float* C, int ldc, int M, int N, int K,
                       float alpha, int relu, void* stream);
+
+/* The QKV projection of one GNN layer as mvm_matcher_forward_views launches it in math mode 3, with the process
+ * defaults of the options: x = X[rows, 256] . W[768, 256]^T + bias, W given as its tf32 planes W_hi / W_lo and,
+ * optionally, as the fp16 planes of wscale * W (W16_hi / W16_lo, both or neither; they select fp16x3).  Columns
+ * [0, 256) of qkv [rows, 768] receive Q = x.  rows a multiple of n_pad (a multiple of 64).
+ *   planes16 = 1 (the fp16x3 attention): K and V leave as half-precision planes of [rows, 256], key-major:
+ *     k_hi = fp16_rn(x_K), k_lo = fp16_rn(x_K - k_hi), v_hi / v_lo the same of x_V; the persistent kernel, whose
+ *     sum order is that of mvm_linear_tc_h16 (fp16 planes) or mvm_linear_tc_presplit (tf32), so x is their output.
+ *   planes16 = 0 (the tf32 attention): qkv[:, 256:512] = rn_tf32(x_K) and k_lo [rows, 256] = rn_tf32(x_K - that);
+ *     v_hi [rows / n_pad, 256, n_pad] = rn_tf32 of V^T by view slot, v_lo its remainder; k_hi is not used.  The
+ *     kernel mvm_linear_tc_presplit would pick.
+ * The K and V thirds of qkv that go to planes are not written. */
+int mvm_qkv_projection(const float* X, const float* W_hi, const float* W_lo, const void* W16_hi, const void* W16_lo,
+                       float wscale, const float* bias, float* qkv, int rows, int n_pad, int planes16, void* k_hi,
+                       void* k_lo, void* v_hi, void* v_lo, void* stream);
 
 /* Math mode of the matcher's GEMMs/attention inside mvm_matcher_forward: 0 = fp32 CUDA cores,
  * 3 = 3xTF32 on the tensor cores (fp32-faithful), 1 = single-pass TF32 (torch 1.10's Ampere default). */
