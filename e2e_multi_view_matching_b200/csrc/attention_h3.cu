@@ -19,9 +19,9 @@ int launch_attention_h3(const float* qkv, const __half* kh, const __half* kl, co
   MVM_REQUIRE(n_pad % 64 == 0 && attn_segs_valid(segs, n_pad, is_cross));
   MvmProfScope prof__(MVM_TAG_ATTN, stream);
   const long long rows = (long long)batch * segs.n_views * n_pad;
-  const CUtensorMap* tK = mvm_get_tmap_2d_f16(kh, rows, 256, 256, attn_wg::BKV);
-  const CUtensorMap* tKlo = mvm_get_tmap_2d_f16(kl, rows, 256, 256, attn_wg::BKV);
-  const CUtensorMap* tV = mvm_get_tmap_2d_f16(vh, rows, 256, 256, attn_wg::BKV);
-  const CUtensorMap* tVlo = mvm_get_tmap_2d_f16(vl, rows, 256, 256, attn_wg::BKV);
+  const CUtensorMap* tK = mvm_get_tmap_2d_f16(kh, rows, 256, 256, attn_wg::Cfg<16>::BKV);
+  const CUtensorMap* tKlo = mvm_get_tmap_2d_f16(kl, rows, 256, 256, attn_wg::Cfg<16>::BKV);
+  const CUtensorMap* tV = mvm_get_tmap_2d_f16(vh, rows, 256, 256, attn_wg::Cfg<16>::BKV);
+  const CUtensorMap* tVlo = mvm_get_tmap_2d_f16(vl, rows, 256, 256, attn_wg::Cfg<16>::BKV);
   return attn_wg::launch<16>(tK, tV, tKlo, tVlo, qkv, out, batch, n_pad, segs, is_cross, stream);
 }

@@ -13,11 +13,11 @@ int launch_attention_tc(const float* qkv, const float* vt, float* out, int batch
   MvmProfScope prof__(MVM_TAG_ATTN, stream);
   const int V = batch * segs.n_views;
   const long long rows = (long long)V * n_pad;
-  const CUtensorMap* tK = mvm_get_tmap_2d(qkv, rows, 768, 768, attn_wg::BKV);
+  const CUtensorMap* tK = mvm_get_tmap_2d(qkv, rows, 768, 768, attn_wg::Cfg<1>::BKV);
   const CUtensorMap* tV = mvm_get_tmap_2d(vt, (long long)V * 256, n_pad, n_pad, attn_wg::HD);
   if (n_pass == 3) {
     MVM_REQUIRE(klo && vtlo);
-    const CUtensorMap* tKlo = mvm_get_tmap_2d(klo, rows, 256, 256, attn_wg::BKV);
+    const CUtensorMap* tKlo = mvm_get_tmap_2d(klo, rows, 256, 256, attn_wg::Cfg<1>::BKV);
     const CUtensorMap* tVlo = mvm_get_tmap_2d(vtlo, (long long)V * 256, n_pad, n_pad, attn_wg::HD);
     return attn_wg::launch<3>(tK, tV, tKlo, tVlo, qkv, out, batch, n_pad, segs, is_cross, stream);
   }

@@ -2,12 +2,14 @@
 // segments.  Reference semantics: attention() superglue.py:87-91, MultiHeadedAttention :94-109, cross source =
 // concatenation of the other views (multi_view_matcher.py:76-78,92-95).  prob[B,4,N,M] is never materialised.
 //
-// One CTA = 128 queries of one (view, head); keys / values stream through in tiles of 64.  288 threads:
-//   warps 0-3, 4-7   two consumer warpgroups, queries [0,64) and [64,128) of the block: S = Q K^T with wgmma (B = K
-//                    tile in shared memory), online softmax on the accumulator registers (a row lives in the four
-//                    threads of a quad), P re-packed in registers as the A operand of O += P V (B = V tile in shared
-//                    memory); O stays in registers until the end
-//   warp 8           TMA producer: the K and V planes of every key tile into ST-deep rings
+// One CTA = 128 queries of one (view, head); keys / values stream through in tiles of BKV (128 in MODE 16, 64 in the
+// tf32 modes).  384 threads:
+//   warps 0-3, 4-7   two consumer warpgroups, queries [0,64) and [64,128) of the block: S = Q K^T with wgmma (A = Q
+//                    fragments in registers, B = K tile in shared memory), online softmax on the accumulator registers
+//                    (a row lives in the four threads of a quad), P re-packed in registers as the A operand of O += P V
+//                    (B = V tile in shared memory); O stays in registers until the end
+//   warps 8-11       the producer warpgroup: one lane of warp 8 issues the TMA loads of the K and V planes of every key
+//                    tile into ST-deep rings
 // Operand arithmetic (MODE):
 //   1   single-pass TF32: K from the fused QKV projection [rows, 768], V^T [view * 256 + h * 64 + d, key] written by the
 //       QKV GEMM epilogue (tf32 wgmma has no transposed B: both operands K-major)
@@ -15,15 +17,17 @@
 //       written by the QKV GEMM epilogue, Q and P are split in registers
 //   16  fp16x3: the same three products on half-precision hi / lo planes (hi = fp16(x), lo = fp16(x - hi): 22 bits like
 //       the tf32 pair) at K = 16 per instruction; K and V planes [rows, 256] come from the QKV GEMM epilogue and V is
-//       read key-major as an MN-major B operand (no transposed copy); Q is split once into hi / lo planes in shared
-//       memory (A operand of S = Q K^T from shared memory)
+//       read key-major as an MN-major B operand (no transposed copy); Q is split once per CTA into hi / lo register
+//       fragments, so S = Q K^T reads only K from shared memory.  128-key tiles halve the per-key cost of what each
+//       tile pays once on a warpgroup's critical path (the waits, the ping-pong barriers, the rescale decision, the
+//       issue); the rescale points of the online softmax and the grouping of the row sums follow the tile, so results
+//       differ from 64-key tiles by reordered fp32 rounding
 // Schedule (MODE 16): inside a warpgroup, S(j+1) = Q K(j+1)^T and O += P(j) V(j) are issued back to back and the
 // softmax of tile j+1 runs while P(j) V(j) is on the tensor cores; across the two warpgroups, named barriers make them
 // take turns issuing (FlashAttention-3 §3.1 ping-pong), so one warpgroup's MMAs cover the other's softmax.  The tf32
-// modes run each tile's S, softmax and P V in order: in MODE 3 the Q split of S(j+1) next to P(j) in flight does not
-// fit the registers; MODE 1 showed no gain beyond run-to-run noise from the ping-pong alone and has not been measured
-// with the overlap inside a warpgroup.
-// Every schedule does the same operations on every output element in the same order: the results are identical.
+// modes run each tile's S, softmax and P V in order; MODE 1 showed no gain beyond run-to-run noise from the ping-pong
+// alone and has not been measured with the overlap inside a warpgroup.
+// For a given tile size, every schedule does the same operations on every output element in the same order.
 #pragma once
 #include <cuda_fp16.h>
 #include "common.cuh"
@@ -32,25 +36,30 @@
 
 namespace attn_wg {
 
-constexpr int BQ = 128, BKV = 64, HD = 64;
-constexpr int NTHREADS = 288;
+constexpr int BQ = 128, HD = 64;
 constexpr int PRODUCER_WARP = 8;
-// named barriers (0 is __syncthreads): warpgroup w may issue its MMAs once PP_BAR + w completes; Q_BAR + w orders a
-// warpgroup's shared-memory Q stores before its first wgmma
-constexpr int PP_BAR = 1, Q_BAR = 3;
+// 384 threads (warps 8-11 are the producer warpgroup) and setmaxnreg 2 x 232 + 40 = the 504 per-thread registers of one
+// SM sub-partition (one warp of each warpgroup).  ptxas budgets a wgmma kernel by whole warpgroups, so 288 threads cap
+// every thread at 168 registers: too few for the Q hi / lo fragments next to the pipelined fp16x3 schedule, and the
+// 3xTF32 instance spilled under that cap.
+constexpr int NTHREADS = 384;
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+// named barriers (0 is __syncthreads): warpgroup w may issue its MMAs once PP_BAR + w completes
+constexpr int PP_BAR = 1;
 
 template <int MODE>
 struct Cfg {
   static constexpr bool F16 = MODE == 16;
   static constexpr bool PIPE = F16;                           // pipelined + ping-pong schedule
+  // keys per tile: S is one m64 x n128 wgmma per k-step in MODE 16 (the tf32 modes keep n64: their operand planes are
+  // twice as wide)
+  static constexpr int BKV = F16 ? 128 : 64;
   static constexpr int PL = MODE == 1 ? 1 : 2;                // operand planes per tile (hi [, lo])
-  static constexpr int PLANE = F16 ? 8192 : 16384;            // [64 x 64]: one fp16 box or two [64 x 32] fp32 boxes
+  static constexpr int PLANE = 16384;                         // [128 x 64] fp16 box, or two [64 x 32] fp32 boxes
   static constexpr int TILE = PL * PLANE;
-  static constexpr int ST = MODE == 3 ? 3 : 4;                // ring depth of K and of V
+  static constexpr int ST = MODE == 1 ? 4 : 3;                // ring depth of K and of V (MODE 16: 192 KB)
   static constexpr int OFF_V = ST * TILE;
-  static constexpr int OFF_Q = 2 * ST * TILE;                 // MODE 16: Q hi, Q lo [128 x 64] fp16, 128B-swizzled
-  static constexpr int QPLANE = BQ * 128;
-  static constexpr int OFF_BAR = OFF_Q + (F16 ? 2 * QPLANE : 0);
+  static constexpr int OFF_BAR = 2 * ST * TILE;
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 };
 
@@ -100,8 +109,10 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
                     const __grid_constant__ Args g) {
   using C_ = Cfg<MODE>;
   constexpr bool F16 = C_::F16, PIPE = C_::PIPE;
-  constexpr int ST = C_::ST, PLANE = C_::PLANE, TILE = C_::TILE;
-  constexpr int KS = F16 ? 4 : 8;                             // K steps over d (S) and over keys (P V)
+  constexpr int ST = C_::ST, PLANE = C_::PLANE, TILE = C_::TILE, BKV = C_::BKV;
+  constexpr int KS = F16 ? 4 : 8;                             // K steps over d (S)
+  constexpr int KP = BKV / (F16 ? 16 : 8);                    // K steps over keys (P V)
+  constexpr int NSC = BKV / 2;                                // S accumulators per thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C_::OFF_BAR);
@@ -127,9 +138,10 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   }
   __syncthreads();
 
-  if (warp == PRODUCER_WARP) {
+  if (warp >= PRODUCER_WARP) {
     // =========================== TMA producer: K(j), V(j) in key-tile order ===========================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+    if (warp == PRODUCER_WARP && lane == 0) {
       tc::prefetch_tmap(&tmK); tc::prefetch_tmap(&tmV);
       if (MODE != 1) { tc::prefetch_tmap(&tmKlo); tc::prefetch_tmap(&tmVlo); }
       int j = 0;
@@ -176,13 +188,14 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   }
 
   // =========================== consumers ===========================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
   const int wg = warp >> 2, wq = warp & 3;
   const int gr = lane >> 2, tq = lane & 3;
   const int lrow = wg * 64 + wq * 16 + gr;                      // query rows of this thread: lrow, lrow + 8
   // Q fragments, raw fp32 (rows past the view are read but never written back; rows past the buffer read as zero).
-  // MODE 16 splits them once into the swizzled hi / lo planes.  The tf32 modes keep them in registers and split them
-  // inside the key-tile loop: when the operand registers were only defined before the loop, ptxas (CUDA 12.9) reused
-  // them inside the loop body and later tiles read stale Q_lo.
+  // MODE 16 splits them once into the hi / lo operand registers; the tf32 modes split them inside the key-tile loop.
+  // When operand registers defined only before the loop are not pinned past the wait that retires their wgmma, ptxas
+  // (CUDA 12.9) reuses them inside the loop body and later tiles read stale Q_lo: retire_s fences them.
   float2 qraw[KS][4];
   {
     const long long total = (long long)gridDim.z * g.n_pad;
@@ -208,23 +221,13 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
       }
     }
   }
+  uint32_t qhi[KS][4], qlo[KS][4];                              // the Q operand of S
   if constexpr (F16) {
-    // element pair (row r, cols 16 kk + 2 tq + 8 (e >> 1)) -> 16-byte chunk 2 kk + (e >> 1) of the 128-byte row r, XOR
-    // r % 8 (= gr): the layout TMA's 128B swizzle gives the K planes
-    uint8_t* sq = smem + C_::OFF_Q + lrow * 128 + 4 * tq;
+    // the f16 k16 A fragment of d [16 kk, 16 kk + 16) is the pair layout qraw[kk] was loaded in
 #pragma unroll
-    for (int kk = 0; kk < KS; ++kk) {
+    for (int kk = 0; kk < KS; ++kk)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        uint32_t hi, lo;
-        split_pack(qraw[kk][e].x, qraw[kk][e].y, hi, lo);
-        const int off = (e & 1) * 1024 + (((2 * kk + (e >> 1)) ^ gr) << 4);
-        *reinterpret_cast<uint32_t*>(sq + off) = hi;
-        *reinterpret_cast<uint32_t*>(sq + C_::QPLANE + off) = lo;
-      }
-    }
-    tc::fence_proxy_async();                                    // generic-proxy stores -> wgmma reads
-    named_bar_sync(Q_BAR + wg, 128);
+      for (int e = 0; e < 4; ++e) split_pack(qraw[kk][e].x, qraw[kk][e].y, qhi[kk][e], qlo[kk][e]);
   }
 
   // online softmax in log2 units (scores * log2(e) / sqrt(d)); row hh of this thread = lrow + 8 hh.  The reference m of
@@ -237,9 +240,8 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   const float scale_l2e = 0.125f * 1.4426950408889634f;
   const int srcA = (lane & ~3) | (tq >> 1), srcB = srcA + 2;   // tf32 P fragments: owners of keys tq and tq + 4
-  float sc[32], fo[2];                                          // fo: rescale of O by the last softmax (1: none)
-  uint32_t qhi[KS][4], qlo[KS][4];                              // tf32 modes: the Q operand of S
-  uint32_t phi[KS][4], plo[KS][4];                              // P of a softmax: the A operand of its P V
+  float sc[NSC], fo[2];                                          // fo: rescale of O by the last softmax (1: none)
+  uint32_t phi[KP][4], plo[KP][4];                              // P of a softmax: the A operand of its P V
 
   auto prep_s = [&] {
     if constexpr (!F16) {
@@ -256,8 +258,8 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
       }
     }
 #pragma unroll
-    for (int i = 0; i < 32; ++i) sc[i] = 0.f;
-    tc::fence_acc<64>(sc);                                      // zeroed before the wgmma fence
+    for (int i = 0; i < NSC; ++i) sc[i] = 0.f;
+    tc::fence_acc<BKV>(sc);                                     // zeroed before the wgmma fence
   };
   // ---- S = Q K^T on the K tile of ring stage st (issue only)
   auto issue_s = [&](int st, uint32_t ph) {
@@ -267,11 +269,10 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 #pragma unroll
     for (int kk = 0; kk < KS; ++kk) {
       if (F16) {
-        const uint32_t qb = tc::smem_u32(smem + C_::OFF_Q + wg * 64 * 128) + kk * 32;
-        const uint64_t dq = tc::make_sw128_desc(qb), dk = tc::make_sw128_desc(kb + kk * 32);
-        tc::wgmma_f16_ss<64>(sc, dq, dk);
-        tc::wgmma_f16_ss<64>(sc, dq, tc::make_sw128_desc(kb + PLANE + kk * 32));
-        tc::wgmma_f16_ss<64>(sc, tc::make_sw128_desc(qb + C_::QPLANE), dk);
+        const uint64_t dk = tc::make_sw128_desc(kb + kk * 32);
+        tc::wgmma_f16_rs<BKV, 0>(sc, qhi[kk], dk);
+        tc::wgmma_f16_rs<BKV, 0>(sc, qhi[kk], tc::make_sw128_desc(kb + PLANE + kk * 32));
+        tc::wgmma_f16_rs<BKV, 0>(sc, qlo[kk], dk);
       } else {
         const uint32_t off = (kk >> 2) * 8192 + (kk & 3) * 32;
         const uint64_t dk = tc::make_sw128_desc(kb + off);
@@ -286,8 +287,9 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   };
   // after the wait that retired the S of ring stage st
   auto retire_s = [&](int st) {
-    tc::fence_acc<64>(sc);
-    if constexpr (!F16) { fence_regs<KS>(qhi); fence_regs<KS>(qlo); }
+    tc::fence_acc<BKV>(sc);
+    fence_regs<KS>(qhi);
+    fence_regs<KS>(qlo);
     tc::mbar_arrive(k_empty + st);
   };
   // ---- O += P V on the V tile of ring stage st (issue only)
@@ -296,7 +298,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     const uint32_t vb = tc::smem_u32(smem + C_::OFF_V + st * TILE);
     tc::wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < KS; ++kk) {
+    for (int kk = 0; kk < KP; ++kk) {
       if (F16) {
         const uint64_t dv = tc::make_sw128_desc(vb + kk * 2048);      // 16 keys x 128 B, V key-major (MN-major B)
         tc::wgmma_f16_rs<64, 1>(o, phi[kk], dv);
@@ -317,15 +319,15 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   // after the wait that retired the P V of ring stage st
   auto retire_pv = [&](int st) {
     tc::fence_acc<64>(o);
-    fence_regs<KS>(phi);
-    fence_regs<KS>(plo);
+    fence_regs<KP>(phi);
+    fence_regs<KP>(plo);
     tc::mbar_arrive(v_empty + st);
   };
   // ---- online softmax of S in place (a row is spread over the four threads of a quad); sets fo, leaves O alone
   auto softmax = [&](int nvalid) {
     if (nvalid < BKV) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
+      for (int i = 0; i < BKV / 8; ++i) {
         const int key = 8 * i + 2 * tq;
         if (key >= nvalid) { sc[4 * i] = -INFINITY; sc[4 * i + 2] = -INFINITY; }
         if (key + 1 >= nvalid) { sc[4 * i + 1] = -INFINITY; sc[4 * i + 3] = -INFINITY; }
@@ -335,7 +337,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     for (int hh = 0; hh < 2; ++hh) {
       float mx = sc[2 * hh];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * hh], sc[4 * i + 2 * hh + 1]));
+      for (int i = 0; i < BKV / 8; ++i) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * hh], sc[4 * i + 2 * hh + 1]));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       mx *= scale_l2e;
@@ -348,7 +350,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
       const float nm = 7.f - m_run[hh];
       float rs = 0.f;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
+      for (int i = 0; i < BKV / 8; ++i) {
         const float p0 = ex2_ftz(fmaf(sc[4 * i + 2 * hh], scale_l2e, nm));
         const float p1 = ex2_ftz(fmaf(sc[4 * i + 2 * hh + 1], scale_l2e, nm));
         sc[4 * i + 2 * hh] = p0;
@@ -373,7 +375,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   // ---- P as the register A operand of O += P V
   auto split_p = [&] {
 #pragma unroll
-    for (int kk = 0; kk < KS; ++kk) {
+    for (int kk = 0; kk < KP; ++kk) {
       if (F16) {
         // the accumulator layout of keys [16 kk, 16 kk + 16) is the k16 A fragment layout
 #pragma unroll
@@ -409,8 +411,8 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   auto finish_pv = [&](int jn) {                                // before stage jn: O += P(jn-1) V(jn-1) can be issued
     tc::wgmma_wait<0>();                                        // P(jn-2) V(jn-2)
     tc::fence_acc<64>(o);
-    fence_regs<KS>(phi);
-    fence_regs<KS>(plo);
+    fence_regs<KP>(phi);
+    fence_regs<KP>(plo);
     if (jn >= 2) tc::mbar_arrive(v_empty + (jn - 2) % ST);
     if (jn >= 1) {
       rescale_o();
