@@ -169,6 +169,8 @@ def lib():
     L.mvm_w8pt.restype = C.c_int
     L.mvm_w8pt.argtypes = [_fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, C.c_int, C.c_int, _fp,
                            _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]
+    L.mvm_w8pt_backward.restype = C.c_int
+    L.mvm_w8pt_backward.argtypes = [_fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, C.c_int, _fp, _fp, _fp, _fp, _fp]
     L.mvm_ransac_essential.restype = C.c_int
     L.mvm_ransac_essential.argtypes = [_fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, C.c_float, C.c_double, C.c_int,
                                        C.c_ulonglong, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]

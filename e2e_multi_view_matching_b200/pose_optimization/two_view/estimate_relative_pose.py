@@ -68,6 +68,40 @@ def _run_w8pt(kpts0, kpts1, intr0, intr1, conf, choose_closest, T_021, determine
     return T, k0n, k1n, cn, pos.bool(), (inl.bool() if inl is not None else None), F
 
 
+class _W8ptFunction(torch.autograd.Function):
+    """_run_w8pt with a gradient for `conf` (mvm_w8pt_backward).  Differentiable outputs: T021 and conf_norm; the
+    normalised keypoints, the masks and F are not.  Keypoints, intrinsics and the target are constants."""
+
+    @staticmethod
+    def forward(ctx, conf, kpts0, kpts1, intr0, intr1, choose_closest, T_021, determine_inliers):
+        T, k0n, k1n, cn, pos, inl, F = _run_w8pt(kpts0, kpts1, intr0, intr1, conf, choose_closest, T_021,
+                                                 determine_inliers)
+        ctx.mark_non_differentiable(k0n, k1n, pos, F, *([inl] if inl is not None else []))
+        B, N, _ = kpts0.shape
+        ctx.choose_closest = bool(choose_closest)
+        ctx.conf_shape, ctx.conf_dtype = conf.shape, conf.dtype
+        Tg = T_021.float().contiguous() if choose_closest else None
+        ctx.save_for_backward(kpts0.float().contiguous(), kpts1.float().contiguous(), _intr4(intr0.to(kpts0.device)),
+                              _intr4(intr1.to(kpts0.device)), conf.reshape(B, N).float().contiguous(), Tg, T)
+        return T, cn, k0n, k1n, pos, inl, F
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gT, gcn, *unused):
+        k0, k1, i0, i1, c, Tg, T = ctx.saved_tensors
+        B, N = c.shape
+        gT = torch.zeros_like(T) if gT is None else gT.float().contiguous()
+        gcn = None if gcn is None else gcn.reshape(B, N).float().contiguous()
+        gc = torch.empty(B, N, dtype=torch.float32, device=c.device)
+        lib = _lib.lib()
+        with torch.cuda.device(c.device):
+            rc = lib.mvm_w8pt_backward(_lib.ptr(k0), _lib.ptr(k1), _lib.ptr(i0), _lib.ptr(i1), _lib.ptr(c), B, N,
+                                       _lib.ptr(Tg), int(ctx.choose_closest), _lib.ptr(T), _lib.ptr(gT), _lib.ptr(gcn),
+                                       _lib.ptr(gc), _lib.stream_ptr())
+        _lib.check(rc, 'mvm_w8pt_backward')
+        return gc.reshape(ctx.conf_shape).to(ctx.conf_dtype), None, None, None, None, None, None, None
+
+
 def find_fundamental(points1, points2, weights):
     """Weighted DLT fundamental matrix (estimate_relative_pose.py:34-82) -> [B,3,3]."""
     B = points1.shape[0]
@@ -76,11 +110,23 @@ def find_fundamental(points1, points2, weights):
 
 
 def estimate_relative_pose_w8pt(kpts0, kpts1, intr0, intr1, confidence, choose_closest=False, T_021=None, determine_inliers=False):
-    """estimate_relative_pose.py:84-128.  Returns (T021 [B,4,4], info) or (None, None)."""
+    """estimate_relative_pose.py:84-128.  Returns (T021 [B,4,4], info) or (None, None).
+
+    Differentiable with respect to `confidence`, in both branches, like the reference: T021 and info["confidence"]
+    carry a graph (the backward is mvm_w8pt_backward); the normalised keypoints, the masks and F do not.  The
+    keypoints, the intrinsics and T_021 are treated as constants -- in the reference's training they are data.  An
+    item with fewer than 8 non-zero confidences gets a NaN gradient: its eight-point solution is not unique.  The
+    default branch selects the cheirality candidate per item (kornia 0.7.0 applies item 0's vote to the whole
+    batch; the reference only calls it with one pair).  When `confidence` does not require grad (or grad mode is
+    off) this is the plain forward launch, and nothing is saved."""
     if kpts0.shape[1] < 8:
         return None, None
-    T, k0n, k1n, cn, pos, inl, F = _run_w8pt(kpts0, kpts1, intr0, intr1, confidence, choose_closest,
-                                             T_021, determine_inliers)
+    if torch.is_grad_enabled() and confidence.requires_grad:
+        T, cn, k0n, k1n, pos, inl, F = _W8ptFunction.apply(confidence, kpts0, kpts1, intr0, intr1, choose_closest,
+                                                           T_021, determine_inliers)
+    else:
+        T, k0n, k1n, cn, pos, inl, F = _run_w8pt(kpts0, kpts1, intr0, intr1, confidence, choose_closest,
+                                                 T_021, determine_inliers)
     info = {"kpts0_norm": k0n, "kpts1_norm": k1n, "confidence": cn.unsqueeze(-1), "inliers": inl,
             "pos_depth_mask": pos, "F": F}
     return T, info

@@ -17,9 +17,10 @@ Built:
   * LogOptimalTransport: autograd.Function over mvm_sinkhorn_train_{forward,backward} -- the exact gradient of the 100
     unrolled iterations (what autograd computes for the reference, superglue.py:143-172), with respect to the scores
     and to bin_score.
-Not built (stated, not hidden): stage 2 of cfg5 (--pose_loss): the gradients through the weighted eight-point, the
-two-view bundle adjustment and the ConfidenceMLP.  run_matcher with opt.pose_loss evaluates those losses (validation)
-but they carry no graph.
+The weighted eight-point is differentiable with respect to the match confidences
+(pose_optimization/two_view/estimate_relative_pose.py, mvm_w8pt_backward), so the pose losses of run_matcher carry a
+graph as far as conf_scores.  Not built (stated, not hidden): the rest of stage 2 of cfg5 (--pose_loss): the backward of
+the ConfidenceMLP, the graph through the train-mode full_output, and train_step with opt.pose_loss (it raises).
 """
 import torch
 
@@ -145,7 +146,9 @@ def compute_gt_matches(opt, data):
 
 def run_matcher(opt, data, matcher):
     """helpers.py:243-260.  Eval mode = the validation pass (train.py:66-68); train mode = the training step, where the
-    match loss carries MatcherTrainFn's graph (the pose losses never do: module docstring)."""
+    match loss carries MatcherTrainFn's graph.  The pose losses carry a graph through the weighted eight-point as far
+    as conf_scores when those require grad; the train-mode conf_scores have none yet (the confidence head's backward
+    is not built), so in train mode the pose losses still reach no parameter."""
     from .pose_optimization.two_view.estimate_relative_pose import run_weighted_8_point
     from .pose_optimization.two_view.compute_pose_error import compute_rotation_error, compute_translation_error_as_angle
     curr_tuple_size = len(data["ids"])

@@ -295,6 +295,19 @@ int mvm_w8pt(const float* kpts0, const float* kpts1, const float* intr0, const f
              float* conf_norm, unsigned char* pos_depth_mask, unsigned char* inliers,
              float* F_out, const int* n_valid, unsigned char* success, void* stream);
 
+/* Backward of mvm_w8pt with respect to conf: one CTA per batch element, fp64 on chip.  The inputs are
+ * mvm_w8pt's (no n_valid: all n keypoints count), its output T021 [B,16], grad_T021 [B,16] and
+ * grad_conf_norm [B,N] (the gradient reaching conf_norm; may be NULL).  The kernel re-runs the
+ * forward's solve and candidate choice and differentiates the reference's steps in closed form: the
+ * smallest right-singular vector of the weighted design matrix, the rank-2 projection,
+ * normalize_transformation and decompose_essential_matrix of the chosen candidate.  Output
+ * grad_conf [B,N].  Items with fewer than 8 non-zero weights (the vector is not unique), or whose
+ * recomputed pose differs from T021 in any bit, get NaN; items with n < 8 get 0. */
+int mvm_w8pt_backward(const float* kpts0, const float* kpts1, const float* intr0, const float* intr1,
+                      const float* conf, int batch, int n, const float* T_gt, int choose_closest,
+                      const float* T021, const float* grad_T021, const float* grad_conf_norm,
+                      float* grad_conf, void* stream);
+
 /* estimate_pose (models/models/utils.py:288-312): OpenCV's findEssentialMat(method=RANSAC) + recoverPose, restated
  * (tests/ransac_oracle.py), one CTA per batch element, fp64 on chip, the whole batch in one launch.
  *   kpts0/1 [B,N,2] pixels (kpts1 already gathered by the matches), intr0/1 [B,4] = fx,fy,cx,cy, n_valid [B] (device,
