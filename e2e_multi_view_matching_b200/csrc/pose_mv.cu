@@ -921,6 +921,12 @@ int mvm_multi_view_ba_obs(const int* pair_a, const int* pair_b, int n_views, int
   g.pscale = (double*)w; w += (size_t)batch * n_pairs * n_pad * 3 * sizeof(double);
   g.xch = (double*)w;
   cudaMemsetAsync(g.ctrs, 0, 1024, stream);
+  // s_rec holds the records of every pair of the tuple: at 8 views (28 pairs, 28 KB) it takes the CTA past the
+  // 48 KB of shared memory a kernel gets without opting in, and the cooperative launch would find no room at all
+  mvm_once_per_device(MVM_ONCE_MVBA, [] {
+    cudaFuncSetAttribute(mvba_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)(MVM_MAX_PAIRS * NPART * sizeof(double)));
+  });
   // the CTAs of a group spin on a software barrier: launch cooperatively so that co-residency of the whole
   // grid is guaranteed by the driver (fails with an error instead of deadlocking when it cannot be)
   {

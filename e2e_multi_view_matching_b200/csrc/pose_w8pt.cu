@@ -368,8 +368,12 @@ __global__ void __launch_bounds__(NT, 2) w8pt_kernel(W8ptArgs a) {
   }
   if (N < 8) {   // fewer than 8 keypoints: no estimate (estimate_relative_pose.py:85-86)
     if (tid < 16) a.T021[b * 16 + tid] = (tid % 5 == 0) ? 1.f : 0.f;
+    // the keypoints are still normalised: the multi-view BA takes every pair's matches, estimated or not
+    // (write_bundle_adjust_problem, bundle_adjust_io.py:193-225), from these buffers
     for (int i = tid; i < N; i += NT) {
-      k0n[2 * i] = 0.f; k0n[2 * i + 1] = 0.f; k1n[2 * i] = 0.f; k1n[2 * i + 1] = 0.f; cn[i] = 0.f;
+      k0n[2 * i] = (k0[2 * i] - cx0) / fx0; k0n[2 * i + 1] = (k0[2 * i + 1] - cy0) / fy0;
+      k1n[2 * i] = (k1[2 * i] - cx1) / fx1; k1n[2 * i + 1] = (k1[2 * i + 1] - cy1) / fy1;
+      cn[i] = 0.f;
       a.pos_depth[(long long)b * NS + i] = 0;
       if (a.inliers) a.inliers[(long long)b * NS + i] = 0;
     }

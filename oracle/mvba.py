@@ -472,11 +472,16 @@ def cams_to_extrinsics(cams):
 # synthetic multi-view scenes + the whole eval_bundle_adjust flow on the CPU
 # ---------------------------------------------------------------------------------------------
 def make_multi_view_scene(seed, n_views, n_kpts, outlier_frac=0.1, noise_px=0.5, width=640, height=480,
-                          f=577.87):
+                          f=577.87, view_counts=None, empty_pairs=()):
     """Landmarks in front of every camera, view 0 = identity, other views rotated <= 12 deg with a
     <= 0.6 m baseline.  Returns pixel keypoints per view, K, GT world->cam poses, and for every pair
-    a<b the matcher-style outputs matches_a [n] (index into view b or -1) and conf [n]."""
+    a<b the matcher-style outputs matches_a [n_a] (index into view b or -1) and conf [n_a].
+    view_counts: keypoints per view (ragged views, each <= n_kpts; None = n_kpts for every view);
+    empty_pairs: pairs (a, b) whose matches are all -1.  With the defaults the scene, random draws
+    included, is the one this function has always produced."""
     from .pose import rodrigues
+    counts = [n_kpts] * n_views if view_counts is None else [int(c) for c in view_counts]
+    assert len(counts) == n_views and max(counts) <= n_kpts
     rng = np.random.default_rng(seed)
     K = np.array([[f, 0, (width - 1) / 2], [0, f, (height - 1) / 2], [0, 0, 1.0]])
     poses = [np.eye(4)]
@@ -502,10 +507,10 @@ def make_multi_view_scene(seed, n_views, n_kpts, outlier_frac=0.1, noise_px=0.5,
             land.append(X)
     land = np.array(land)
     kpts, ids = [], []
-    for T in poses:
-        sel = rng.permutation(len(land))[:n_kpts]
+    for T, n_v in zip(poses, counts):
+        sel = rng.permutation(len(land))[:n_v]
         q = land[sel] @ T[:3, :3].T + T[:3, 3]
-        px = (q @ K.T)[:, :2] / q[:, 2:3] + noise_px * rng.standard_normal((n_kpts, 2))
+        px = (q @ K.T)[:, :2] / q[:, 2:3] + noise_px * rng.standard_normal((n_v, 2))
         kpts.append(px.astype(np.float32))
         ids.append(sel)
     matches, conf = {}, {}
@@ -513,10 +518,12 @@ def make_multi_view_scene(seed, n_views, n_kpts, outlier_frac=0.1, noise_px=0.5,
         for a in range(b):
             lut = {l: j for j, l in enumerate(ids[b])}
             m = np.array([lut.get(l, -1) for l in ids[a]], dtype=np.int64)
-            c = rng.uniform(0.5, 1.0, n_kpts)
-            bad = (rng.uniform(size=n_kpts) < outlier_frac) & (m >= 0)
-            m[bad] = rng.integers(0, n_kpts, int(bad.sum()))
+            c = rng.uniform(0.5, 1.0, counts[a])
+            bad = (rng.uniform(size=counts[a]) < outlier_frac) & (m >= 0)
+            m[bad] = rng.integers(0, counts[b], int(bad.sum()))
             c[bad] = rng.uniform(0.05, 0.3, int(bad.sum()))
+            if (a, b) in empty_pairs:
+                m[:] = -1
             matches[(a, b)] = m
             conf[(a, b)] = c.astype(np.float32)
     return {'kpts': kpts, 'K': K.astype(np.float32), 'poses': np.array(poses), 'matches': matches, 'conf': conf}
@@ -560,4 +567,4 @@ def multi_view_pipeline(scene, conf_thresh=0.0, n_it2=10, max_iterations=50, use
     pb = build_problem(T, pm, extr0)
     cams, pts, info = solve_schur(pb, max_iterations=max_iterations)
     return {'rel': rel, 'extr_tree': extr_tree, 'extr_init': extr0, 'extr': cams_to_extrinsics(cams), 'info': info, 'pairs': info_all,
-            'weight': weight}
+            'weight': weight, 'problem': pb}

@@ -32,6 +32,39 @@ def test_angle_axis_jacobian_and_roundtrip():
         assert np.abs(M.R_to_angle_axis(M.angle_axis_to_R(w)) - w).max() < 1e-12
 
 
+def _scene_digest(sc):
+    import hashlib
+    h = hashlib.sha256()
+    for k in sc['kpts']:
+        h.update(np.ascontiguousarray(k).tobytes())
+    h.update(sc['K'].tobytes())
+    h.update(sc['poses'].tobytes())
+    for key in sorted(sc['matches']):
+        h.update(sc['matches'][key].tobytes())
+        h.update(sc['conf'][key].tobytes())
+    return h.hexdigest()[:16]
+
+
+@pytest.mark.parametrize('args,kw,digest', [((1, 3, 60), dict(outlier_frac=0.0), '6e8f9b6c84a7385e'),
+                                            ((2, 5, 100), dict(outlier_frac=0.1), 'aa84f8b954d1d014'),
+                                            ((7, 4, 120), dict(outlier_frac=0.0, noise_px=0.0), '1ae23e0574359342')])
+def test_scene_generator_is_unchanged(args, kw, digest):
+    """The scenes the GPU parity tests use are pinned: the ragged-view and empty-pair options of
+    make_multi_view_scene leave the default scene (and its random draws) exactly as before, and
+    spelling the defaults out gives the same scene."""
+    assert _scene_digest(M.make_multi_view_scene(*args, **kw)) == digest
+    assert _scene_digest(M.make_multi_view_scene(*args, view_counts=[args[2]] * args[1], empty_pairs=(), **kw)) == digest
+
+
+def test_scene_ragged_views_and_empty_pairs():
+    sc = M.make_multi_view_scene(5, 4, 300, view_counts=[300, 200, 7, 256], empty_pairs=[(1, 3)])
+    assert [k.shape[0] for k in sc['kpts']] == [300, 200, 7, 256]
+    for (a, b), m in sc['matches'].items():
+        assert m.shape == sc['conf'][(a, b)].shape == (sc['kpts'][a].shape[0],)
+        assert m.max() < sc['kpts'][b].shape[0]
+        assert (m < 0).all() == ((a, b) == (1, 3))
+
+
 def test_pipeline_recovers_poses():
     sc = M.make_multi_view_scene(3, 4, 80, outlier_frac=0.0, noise_px=0.2)
     out = M.multi_view_pipeline(sc)
