@@ -14,12 +14,20 @@
 // One CTA computes 128 x BN output tiles:
 //   warps 0-3, 4-7   two consumer warpgroups, tile rows [0,64) and [64,128): A fragments from the 128B-swizzled shared
 //                    tile -> hi / lo in registers -> wgmma m64 x BN (B = the W planes, shared-memory descriptors), fp32
-//                    accumulators in registers; then the epilogue straight from the accumulators.  With BN = 128 the
+//                    accumulators in registers; then the epilogue (below).  With BN = 128 the
 //                    wgmma of k-block kt are issued before the A fragments of kt + 1 are split, so the split runs under
-//                    them (two fragment sets in registers, raised to 232 per thread by setmaxnreg), and the epilogue
-//                    loads its bias / residual operands in batches
+//                    them (two fragment sets in registers, raised to 232 per thread by setmaxnreg)
 //   warps 8-11       the producer warpgroup (40 registers): one lane of warp 8 issues the
 //                    TMA loads of A [128 x BK] (fp32) and the W planes [BN x 128 B] into a STAGES-deep ring
+// Epilogue of the persistent instances (128 columns, pre-split W planes: Cfg::STAGED): the consumers finish the tile in
+// rounds of one 16 KB TMA box ([128 x 32] fp32 or [128 x 64] of one fp16 plane), written swizzled into one of two
+// staging buffers after the ring, and go back to the mainloop of the next tile after the last round; lane 0 of warp 9
+// (the storer) drains each round by a TMA store and, for a residual, loads the residual box of the round that will use
+// that buffer next, so the residual arrives in shared memory before it is needed (in place R == C stays correct: a box
+// is loaded before the same box is stored, and tiles do not overlap).  The tensor maps carry the logical M x N, so rows
+// >= M and columns N .. ldc are never written.  The score matrices (rows of n + 1 floats: not 16-byte aligned), the V^T
+// output of the tf32 attention, C or R with only 8-byte alignment, and the other instances keep the direct stores
+// from the accumulators, with the bias / residual operands of eight column groups loaded at once.
 // The tile schedule is static: with `persistent` one CTA per SM walks the tiles (the producer fills the ring for the
 // next tile under the epilogue of the current one), otherwise one tile per CTA.  Both issue the same instructions per
 // tile, so their results are bit-identical.
@@ -53,7 +61,12 @@ struct Cfg {
   static constexpr int STAGE_BYTES = A_BYTES + PLANES * W_PLANE;
   static constexpr int TMA_BYTES = A_BYTES + (WM == W_RAW ? 1 : PLANES) * W_PLANE;
   static constexpr int STAGES = (196608 / STAGE_BYTES) < 6 ? (196608 / STAGE_BYTES) : 6;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  // the persistent instances (128-column tiles, pre-split W planes) stage their output tiles for TMA stores in two
+  // [128 rows x 128 B] buffers after the ring
+  static constexpr bool STAGED = BN == 128 && NPASS == 3 && WM != W_RAW;
+  static constexpr int OUT_BYTES = STAGED ? 2 * 16384 : 0;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + OUT_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 232448, "over the sm_90 dynamic shared memory opt-in limit");
 };
 
 struct GArgs {
@@ -76,6 +89,14 @@ struct GArgs {
   // writes its partial product to rows [s * tiles_m * BM, ...) of C (a slab buffer that a small kernel sums afterwards,
   // in fixed order).  1 = off.
   int ksplit;
+  // 1: output tiles leave through the staging buffers by TMA stores (maps in StoreMaps), all but the V^T columns
+  int stage;
+};
+
+// Tensor maps of the staged epilogue: C [rows, N] fp32 (rows = M, or the split-K slabs), the residual R [M, N], and the
+// output planes [M, 256]: KH16, KL16, VH16, VL16 (fp16 boxes [128 x 64]) or KLO in p[0] (fp32 boxes [128 x 32]).
+struct StoreMaps {
+  CUtensorMap c, r, p[4];
 };
 
 // SCORE mode: one launch computes every (pair, tuple) score matrix  scores = mdesc_a . mdesc_b^T * alpha  into the
@@ -98,6 +119,18 @@ __device__ __forceinline__ void split_pack_h(float x0, float x1, uint32_t& hi, u
   hi = *reinterpret_cast<const uint32_t*>(&h);
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
+// shared-memory accesses of the staging buffers (the aligned dynamic-smem pointer is generic to the compiler)
+__device__ __forceinline__ void sts_f2(uint32_t a, float2 v) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v.x), "f"(v.y) : "memory");
+}
+__device__ __forceinline__ void sts_u32(uint32_t a, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
+}
+__device__ __forceinline__ float2 lds_f2(uint32_t a) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+  return v;
+}
 // A-fragment registers of an issued wgmma stay live (and unchanged) until this point, after the wait that retires it
 __device__ __forceinline__ void fence_afrag(uint32_t (&a)[4][4]) {
 #pragma unroll
@@ -110,17 +143,22 @@ template <int BN, int NPASS, int WM, bool SCORE>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                const __grid_constant__ CUtensorMap tmWhi, const __grid_constant__ CUtensorMap tmWlo,
-               const __grid_constant__ GArgs g, const __grid_constant__ ScoreTab st) {
+               const __grid_constant__ GArgs g, const __grid_constant__ ScoreTab st,
+               const __grid_constant__ StoreMaps sm) {
   using C_ = Cfg<BN, NPASS, WM>;
   static_assert(NPASS == 3 || WM == W_RAW, "single pass reads the raw W");
   constexpr int BK = C_::BK, STAGES = C_::STAGES, A_BYTES = C_::A_BYTES, W_PLANE = C_::W_PLANE;
   constexpr int STAGE_BYTES = C_::STAGE_BYTES;
   constexpr int KSTEPS = 4;                                   // 4 x (K = 8 tf32 | K = 16 halves) per k-block
   constexpr bool PIPE = BN == 128;                            // pipelined mainloop (see the consumers)
+  constexpr bool STAGED = C_::STAGED && !SCORE;               // staged epilogue (when g.stage)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);   // [STAGES] TMA landed
+  uint8_t* obuf = smem + STAGES * STAGE_BYTES;                                  // [2][16 KB] output staging
+  uint64_t* full = reinterpret_cast<uint64_t*>(obuf + C_::OUT_BYTES);          // [STAGES] TMA landed
   uint64_t* empty = full + STAGES;                                              // [STAGES] both warpgroups done (256)
+  uint64_t* ostaged = empty + STAGES;      // [2] staging buffer written by all 256 consumer threads
+  uint64_t* ofree = ostaged + 2;           // [2] staging buffer drained by its store (and holding its residual box)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nk = SCORE ? g.K / BK : g.K / BK / g.ksplit;     // k-blocks per tile (per K slice)
@@ -139,12 +177,27 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       w_row = (bi * st.n_views + st.b[p]) * st.n_pad + n0;
     }
   };
+  // How the staged epilogue writes the tile at column n0, in rounds of one 16 KB box per staging buffer (the same
+  // precedence as the direct stores below): 0 = fp32 C, four [128 x 32] boxes; 1 = the fp16 K / V planes, hi and lo of
+  // two [128 x 64] halves; 2 = the tf32 K planes, rn_tf32 in C and the remainder in KLO, of four [128 x 32] quarters;
+  // -1 = not staged (V^T, direct stores)
+  auto tile_kind = [&](int n0) {
+    if (g.VT && n0 >= g.vt_col0) return -1;
+    if (g.KH16 && n0 >= 256) return 1;
+    if (g.KLO && n0 >= 256 && n0 < 512) return 2;
+    return 0;
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       tc::mbar_init(full + s, 1);
       tc::mbar_init(empty + s, 256);
     }
+    if (STAGED)
+      for (int b = 0; b < 2; ++b) {
+        tc::mbar_init(ostaged + b, 256);
+        tc::mbar_init(ofree + b, 1);
+      }
     tc::fence_barrier_init();
   }
   __syncthreads();
@@ -152,6 +205,54 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp >= PRODUCER_WARP) {
     // ================================ TMA producer ================================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+    if (STAGED && g.stage && warp == PRODUCER_WARP + 1 && lane == 0) {
+      // ---- storer: drains each staged round by a TMA store, then hands its buffer back for round u + 2 (loading
+      // that round's residual box first, if any: a residual is only staged into a plain fp32 C)
+      tc::prefetch_tmap(&sm.c);
+      if (g.R) tc::prefetch_tmap(&sm.r);
+      if (g.KH16)
+        for (int i = 0; i < 4; ++i) tc::prefetch_tmap(&sm.p[i]);
+      if (g.KLO) tc::prefetch_tmap(&sm.p[0]);
+      auto hand_back = [&](uint32_t u, int tile, int q) {
+        uint64_t* bar = ofree + (u & 1);
+        if (!g.R) {
+          tc::mbar_arrive(bar);
+        } else if (tile < n_tiles) {
+          int m0, n0, a_row, w_row, prob;
+          decode(tile, m0, n0, a_row, w_row, prob);
+          tc::mbar_arrive_expect_tx(bar, 16384);
+          tc::tma_load_2d(obuf + (u & 1) * 16384, &sm.r, bar, n0 + 32 * q, m0);
+        }
+      };
+      hand_back(0, blockIdx.x, 0);
+      hand_back(1, blockIdx.x, 1);
+      uint32_t u = 0;
+      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        int m0, n0, a_row, w_row, prob;
+        decode(tile, m0, n0, a_row, w_row, prob);
+        const int kind = tile_kind(n0);
+        if (kind < 0) continue;
+        const int rounds = kind == 2 ? 8 : 4;
+        for (int j = 0; j < rounds; ++j, ++u) {
+          const uint8_t* buf = obuf + (u & 1) * 16384;
+          tc::mbar_wait(ostaged + (u & 1), (u >> 1) & 1);
+          if (kind == 0) {
+            tc::tma_store_2d(&sm.c, buf, n0 + 32 * j, m0 + prob * g.tiles_m * BM);
+          } else if (kind == 1) {
+            const bool v = n0 >= 512;
+            tc::tma_store_2d(&sm.p[(v ? 2 : 0) + (j & 1)], buf, n0 - (v ? 512 : 256) + 64 * (j >> 1), m0);
+          } else {
+            if (j & 1) tc::tma_store_2d(&sm.p[0], buf, n0 - 256 + 32 * (j >> 1), m0);
+            else tc::tma_store_2d(&sm.c, buf, n0 + 32 * (j >> 1), m0);
+          }
+          tc::tma_store_commit();
+          tc::tma_store_wait_read<0>();
+          // with a residual every tile has 4 rounds: round u + 2 is quarter j + 2 of this tile or j - 2 of the next
+          hand_back(u + 2, j < 2 ? tile : tile + gridDim.x, (j + 2) & 3);
+        }
+      }
+      tc::tma_store_wait_all();
+    }
     if (warp == PRODUCER_WARP && lane == 0) {
       tc::prefetch_tmap(&tmA); tc::prefetch_tmap(&tmA2); tc::prefetch_tmap(&tmWhi); tc::prefetch_tmap(&tmWlo);
       uint32_t it = 0;
@@ -273,7 +374,50 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (NPASS == 3) fence_afrag(alo);
   };
 
-  uint32_t it = 0;
+  // one staged round: the column groups [i0, i0 + ni) of both rows of this thread, finished in the order of the direct
+  // stores (rounded products and sums, never contracted), written into staging buffer u & 1 in the TMA box's 128B
+  // swizzle (16-byte chunk c of row r at c ^ (r & 7): each warp writes 8 rows x 32 B, or 8 rows x 16 B of fp16,
+  // free of bank conflicts).  mode 0: fp32 pairs (+ the residual the storer loaded into the buffer); mode 1: the fp16
+  // hi (plane 0) or lo (plane 1) of the pairs; mode 2: rn_tf32 (plane 0) or the tf32 remainder (plane 1).
+  auto stage_round = [&](uint32_t u, int n0, int i0, int ni, int mode, int plane) {
+    const uint32_t buf = tc::smem_u32(obuf + (u & 1) * 16384);
+    float2 bv[8];
+#pragma unroll
+    for (int c = 0; c < ni; ++c) {
+      const int n = n0 + 8 * (i0 + c) + 2 * tq;
+      bv[c] = g.bias ? make_float2(__ldg(g.bias + n), __ldg(g.bias + n + 1)) : make_float2(0.f, 0.f);
+    }
+    tc::mbar_wait(ofree + (u & 1), (u >> 1) & 1);
+#pragma unroll
+    for (int c = 0; c < ni; ++c) {
+      const int i = i0 + c;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = row0 + 8 * hh;
+        float x0 = __fmul_rn(g.alpha, acc[4 * i + 2 * hh]), x1 = __fmul_rn(g.alpha, acc[4 * i + 2 * hh + 1]);
+        if (g.bias) { x0 = __fadd_rn(x0, bv[c].x); x1 = __fadd_rn(x1, bv[c].y); }
+        if (g.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+        if (mode == 1) {
+          uint32_t hi, lo;
+          split_pack_h(x0, x1, hi, lo);
+          sts_u32(buf + r * 128 + ((c ^ (r & 7)) << 4) + 4 * tq, plane ? lo : hi);
+        } else {
+          const uint32_t p = buf + r * 128 + (((2 * c + (tq >> 1)) ^ (r & 7)) << 4) + 8 * (tq & 1);
+          if (mode == 2) {
+            const float h0 = tf32_hi(x0), h1 = tf32_hi(x1);
+            sts_f2(p, plane ? make_float2(tf32_hi(x0 - h0), tf32_hi(x1 - h1)) : make_float2(h0, h1));
+          } else {
+            if (g.R) { const float2 rv = lds_f2(p); x0 = __fadd_rn(x0, rv.x); x1 = __fadd_rn(x1, rv.y); }
+            sts_f2(p, make_float2(x0, x1));
+          }
+        }
+      }
+    }
+    tc::fence_proxy_async();      // generic-proxy writes -> visible to the TMA store (async proxy)
+    tc::mbar_arrive(ostaged + (u & 1));
+  };
+
+  uint32_t it = 0, u = 0;         // u: staged rounds so far (buffer u & 1)
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     int m0, n0, a_row, w_row, prob;
     decode(tile, m0, n0, a_row, w_row, prob);
@@ -335,6 +479,25 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
       continue;
+    }
+    if constexpr (STAGED) {
+      const int kind = g.stage ? tile_kind(n0) : -1;
+      if (kind >= 0) {
+        // the storer drains each round while the next is written and, after the last, while the mainloop of the
+        // next tile runs; rows >= M and columns beyond N lie outside the tensor maps and are never stored
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          if (kind == 1) {
+            if (j < 4) stage_round(u + j, n0, 8 * (j >> 1), 8, 1, j & 1);
+          } else if (kind == 2) {
+            stage_round(u + j, n0, 4 * (j >> 1), 4, 2, j & 1);
+          } else if (j < 4) {
+            stage_round(u + j, n0, 4 * j, 4, 0, 0);
+          }
+        }
+        u += kind == 2 ? 8 : 4;
+        continue;
+      }
     }
     // store the finished pair (x0, x1) of row m, columns n, n + 1 in the layout(s) the caller asked for
     auto put = [&](int m, int n, float x0, float x1) {
@@ -423,17 +586,26 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
 template <int BN, int NPASS, int WM, bool SCORE>
 int launch_wg(const CUtensorMap* tA, const CUtensorMap* tA2, const CUtensorMap* tWhi, const CUtensorMap* tWlo,
-              const GArgs& g, const ScoreTab& st, long long n_tiles, bool persistent, cudaStream_t stream) {
+              const GArgs& g, const ScoreTab& st, long long n_tiles, bool persistent, cudaStream_t stream,
+              const StoreMaps& sm) {
   using C_ = Cfg<BN, NPASS, WM>;
   if (!tA || !tA2 || !tWhi || !tWlo) return MVM_ERR_LAUNCH;
   if (n_tiles <= 0) return MVM_OK;
   // cheap and idempotent: set on every launch (per-device attribute)
-  cudaFuncSetAttribute(gemm_wg_kernel<BN, NPASS, WM, SCORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM_BYTES);
+  if (cudaFuncSetAttribute(gemm_wg_kernel<BN, NPASS, WM, SCORE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           C_::SMEM_BYTES) != cudaSuccess)
+    return MVM_ERR_LAUNCH;
   const int n_sm = mvm_dev_info().n_sm;
   const int grid = (persistent && n_tiles > n_sm) ? n_sm : (int)n_tiles;
-  gemm_wg_kernel<BN, NPASS, WM, SCORE><<<grid, NTHREADS, C_::SMEM_BYTES, stream>>>(*tA, *tA2, *tWhi, *tWlo, g, st);
+  gemm_wg_kernel<BN, NPASS, WM, SCORE><<<grid, NTHREADS, C_::SMEM_BYTES, stream>>>(*tA, *tA2, *tWhi, *tWlo, g, st, sm);
   MVM_CHECK_LAUNCH();
   return MVM_OK;
+}
+
+StoreMaps no_store_maps() {
+  StoreMaps none;
+  memset(&none, 0, sizeof(none));
+  return none;
 }
 
 GArgs make_args(const GemmDesc& d, float* VT, int vt_col0, int n_pad, float* KLO, float* VTLO, int bn) {
@@ -461,7 +633,7 @@ int launch_cfg(const GemmDesc& d, float* VT, int vt_col0, int n_pad, float* KLO,
   const CUtensorMap* tWlo = WM == W_TF32 ? mvm_get_tmap_2d(d.Wlo, d.N, d.K, d.ldw, BN) : tW;
   const GArgs g = make_args(d, VT, vt_col0, n_pad, KLO, VTLO, BN);
   return launch_wg<BN, NPASS, WM, false>(tA, tA2, tW, tWlo, g, no_scores(), (long long)g.tiles_m * g.tiles_n, persistent,
-                                         stream);
+                                         stream, no_store_maps());
 }
 
 
@@ -617,15 +789,35 @@ int launch_gemm_tc_persist(const GemmDesc& d, float* VT, int vt_col0, int n_pad,
     g.KH16 = (__half*)hp->kh; g.KL16 = (__half*)hp->kl; g.VH16 = (__half*)hp->vh; g.VL16 = (__half*)hp->vl;
   }
   const long long n_tiles = (long long)g.tiles_m * g.tiles_n * ksplit;
+  // Output tiles leave by TMA stores when every buffer they touch can be a TMA base (16-byte aligned; gemm_desc_valid
+  // also accepts an 8-byte aligned C and R, which keep the direct stores), and a residual only with a plain fp32 C.
+  StoreMaps sm = no_store_maps();
+  const void* planes[4] = {g.KH16, g.KL16, g.VH16, g.VL16};
+  bool stage = mvm_aligned(g.C, 16) && mvm_aligned(g.R, 16) && mvm_aligned(g.KLO, 16) && (!g.VT || g.vt_col0 % 128 == 0) &&
+               (!g.R || (!g.KH16 && !g.KLO && !g.VT));
+  for (const void* p : planes) stage = stage && mvm_aligned(p, 16);
+  if (stage) {
+    const CUtensorMap* c = mvm_get_tmap_2d(g.C, (long long)(ksplit - 1) * g.tiles_m * BM + g.M, g.N, g.ldc, BM);
+    const CUtensorMap* r = g.R ? mvm_get_tmap_2d(g.R, g.M, g.N, g.ldr, BM) : c;
+    if (!c || !r) return MVM_ERR_LAUNCH;
+    sm.c = *c; sm.r = *r;
+    for (int i = 0; i < 4; ++i) {
+      const CUtensorMap* p = g.KH16 ? mvm_get_tmap_2d_f16(planes[i], g.M, 256, 256, BM)
+                                    : g.KLO && i == 0 ? mvm_get_tmap_2d(g.KLO, g.M, 256, 256, BM) : c;
+      if (!p) return MVM_ERR_LAUNCH;
+      sm.p[i] = *p;
+    }
+    g.stage = 1;
+  }
   if (f16) {
     g.alpha = d.alpha / d.wscale;
     const CUtensorMap* tWhi = mvm_get_tmap_2d_f16(d.Whi16, d.N, d.K, d.ldw, 128);
     const CUtensorMap* tWlo = mvm_get_tmap_2d_f16(d.Wlo16, d.N, d.K, d.ldw, 128);
-    return launch_wg<128, 3, W_F16, false>(tA, tA2, tWhi, tWlo, g, no_scores(), n_tiles, true, stream);
+    return launch_wg<128, 3, W_F16, false>(tA, tA2, tWhi, tWlo, g, no_scores(), n_tiles, true, stream, sm);
   }
   const CUtensorMap* tWhi = mvm_get_tmap_2d(d.Whi, d.N, d.K, d.ldw, 128);
   const CUtensorMap* tWlo = mvm_get_tmap_2d(d.Wlo, d.N, d.K, d.ldw, 128);
-  return launch_wg<128, 3, W_TF32, false>(tA, tA2, tWhi, tWlo, g, no_scores(), n_tiles, true, stream);
+  return launch_wg<128, 3, W_TF32, false>(tA, tA2, tWhi, tWlo, g, no_scores(), n_tiles, true, stream, sm);
 }
 
 int launch_splitk_reduce(const float* slabs, float* C, int M, int N, int ldc, int ksplit, cudaStream_t stream) {
@@ -662,5 +854,5 @@ int launch_score_gemm_tc(const float* mdesc, float* hi, float* lo, int n_pad, co
   g.K = 256; g.K1 = 256; g.alpha = alpha; g.ksplit = 1;
   g.tiles_m = mvm_div_up(max_m, BM); g.tiles_n = mvm_div_up(max_n, 128);
   const long long n_tiles = (long long)g.tiles_m * g.tiles_n * tab.n_pairs * batch;
-  return launch_wg<128, 3, W_TF32, true>(tA, tA, tWhi, tWlo, g, st, n_tiles, true, stream);
+  return launch_wg<128, 3, W_TF32, true>(tA, tA, tWhi, tWlo, g, st, n_tiles, true, stream, no_store_maps());
 }

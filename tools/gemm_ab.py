@@ -1,5 +1,7 @@
 """Per-shape timing of the fp16x3 layer GEMM (gemm_wg_kernel<128, 3, W_F16>) at the shapes of one cfg3 step
-(14 tuples x 5 views x 1024 keypoints = 71680 rows; the confidence head runs on twice as many rows).
+(14 tuples x 5 views x 1024 keypoints = 71680 rows; the confidence head runs on twice as many rows).  'qkv' is the
+projection as a plain fp32 [M, 768] output; 'qkv.planes' is the matcher's own launch (ops.qkv_projection, planes='fp16'):
+Q in fp32, K and V as the fp16 hi / lo planes of the attention.
 
 Kernel durations come from CUPTI (torch.profiler, CUDA activities) with the L2 flushed before every launch.  For each
 shape the script prints the median duration, the algorithmic rate (2 M N K per launch; fp16x3 issues three tensor-core
@@ -21,7 +23,8 @@ SHAPES = [('qkv', M, 256, 0, 768, 'bias'),
           ('mlp.0', M, 256, 256, 512, 'concat+bias+relu'),
           ('mlp.2', M, 512, 0, 256, 'bias+residual'),
           ('conf.0', 2 * M, 512, 0, 512, 'bias+relu'),
-          ('conf.1', 2 * M, 512, 0, 256, 'bias')]
+          ('conf.1', 2 * M, 512, 0, 256, 'bias'),
+          ('qkv.planes', M, 256, 0, 768, 'bias+fp16 planes')]
 
 
 def smi(query):
@@ -61,9 +64,16 @@ def main():
         b = torch.randn(N, generator=g).cuda()
         r = torch.randn(rows, N, generator=g).cuda() if 'residual' in epi else None
         cases.append((name, rows, K1 + K2, N, epi, dict(a=a, w=w, bias=b, a2=a2, residual=r, relu='relu' in epi)))
-    for *_, kw in cases:                        # warm-up: module load, tensor maps
-        for _ in range(3):
+    qkv_out = torch.empty(M, 768, device='cuda')
+
+    def run(name, kw):
+        if name == 'qkv.planes':
+            ops.qkv_projection(kw['a'], kw['w'], kw['bias'], 1024, planes='fp16', out=qkv_out)
+        else:
             ops.linear(tc_passes='h16', **kw)
+    for name, *_, kw in cases:                  # warm-up: module load, tensor maps
+        for _ in range(3):
+            run(name, kw)
     torch.cuda.synchronize()
     sampler = ClockSampler()
     sampler.start()
@@ -72,7 +82,7 @@ def main():
         for name, *_, kw in cases:
             for _ in range(args.reps):
                 flush.zero_()
-                ops.linear(tc_passes='h16', **kw)
+                run(name, kw)
         torch.cuda.synchronize()
     sampler.stop.set()
     sampler.join()
