@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, 'libmvm_b200.so')
 
 MVM_MAX_LAYERS = 64
 MVM_MAX_VIEWS = 8
+MVM_SUPERPOINT_MAX_SELECT = 16384
 
 _fp = C.c_void_p  # device pointers travel as integers
 
@@ -208,6 +209,10 @@ def lib():
                                        C.c_size_t, _fp]
     L.mvm_superpoint_sample.restype = C.c_int
     L.mvm_superpoint_sample.argtypes = [_fp, _fp, C.c_int, C.c_int, C.c_int, _fp, _fp]
+    L.mvm_superpoint_select.restype = C.c_int
+    L.mvm_superpoint_select.argtypes = [_fp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _fp, _fp, _fp, _fp]
+    L.mvm_superpoint_sample_batch.restype = C.c_int
+    L.mvm_superpoint_sample_batch.argtypes = [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp, _fp]
     L.mvm_match_loss_forward.restype = C.c_int
     L.mvm_match_loss_forward.argtypes = [_fp, _fp, _fp, C.c_int, C.c_int, _fp, _fp, _fp]
     L.mvm_match_loss_backward.restype = C.c_int

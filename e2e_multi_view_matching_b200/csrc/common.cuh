@@ -55,7 +55,7 @@ bool* mvm_attr_flag(int slot);   // flag of (current device, slot); call with mv
 enum MvmOnceSlot { MVM_ONCE_SINKHORN_CL = 0, MVM_ONCE_SINKHORN_EXP, MVM_ONCE_SINKHORN_LOG, MVM_ONCE_ATTN_TC,
                    MVM_ONCE_ATTN_SIMT, MVM_ONCE_GEMM_TC, MVM_ONCE_GEMM_PERSIST, MVM_ONCE_GEMM_SCORE, MVM_ONCE_KENC,
                    MVM_ONCE_MVBA, MVM_ONCE_ATTN_H3, MVM_ONCE_ATTN_H3S, MVM_ONCE_ATTN_BWD, MVM_ONCE_SINKHORN_TRAIN,
-                   MVM_N_ONCE = 32 };
+                   MVM_ONCE_SP_SELECT, MVM_N_ONCE = 32 };
 template <class F>
 static inline void mvm_once_per_device(int slot, F&& f) {
   std::lock_guard<std::mutex> g(mvm_attr_mutex());

@@ -17,6 +17,8 @@
 //   sp_nms_step kernels   the reference's three-round suppression, statement for statement
 //   sp_l2norm_kernel      per-pixel L2 normalisation of the dense descriptors (:216)
 //   sp_sample_kernel      bilinear sampling (grid_sample, align_corners=True) at the keypoints + L2 normalisation (:86-100)
+//   sp_sample_batch_kernel  the same sampling for [B, K] keypoints into [B, 256, K] descriptors
+//   sp_select_kernel      threshold + border mask + exact top-k of every image of a batch in one launch (radix select)
 #include "../../include/mvm_b200.h"
 #include "common.cuh"
 #include "kernels.cuh"
@@ -220,14 +222,13 @@ __global__ void __launch_bounds__(256) sp_l2norm_kernel(float* __restrict__ d, l
   for (int k = 0; k < 8; ++k) p[lane + 32 * k] = v[k] * inv;
 }
 
-// sample_descriptors (superpoint.py:86-100): keypoints (x, y) in pixels of the s = 8 times larger image, bilinear
-// grid_sample with align_corners=True on the dense [h, w, 256] map, L2 normalisation; out [256, n] channel-first.
-__global__ void __launch_bounds__(256) sp_sample_kernel(const float* __restrict__ dense, const float* __restrict__ kpts,
-                                                        float* __restrict__ out, int n, int h, int w) {
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (warp >= n) return;
+// sample_descriptors (superpoint.py:86-100) for one keypoint, one warp: keypoint (x, y) in pixels of the s = 8 times
+// larger image, bilinear grid_sample with align_corners=True on the dense [h, w, 256] map, L2 normalisation; channel c
+// goes to out[c * stride].  Both sampling kernels run this code, so their descriptors are the same bits.
+__device__ __forceinline__ void sp_sample_point(const float* __restrict__ dense, const float* __restrict__ kp, int h,
+                                                int w, int lane, float* __restrict__ out, long long stride) {
   const float s = 8.f;
-  float kx = kpts[2 * warp] - s / 2 + 0.5f, ky = kpts[2 * warp + 1] - s / 2 + 0.5f;
+  float kx = kp[0] - s / 2 + 0.5f, ky = kp[1] - s / 2 + 0.5f;
   kx /= (w * s - s / 2 - 0.5f);
   ky /= (h * s - s / 2 - 0.5f);
   kx = kx * 2 - 1;
@@ -251,7 +252,230 @@ __global__ void __launch_bounds__(256) sp_sample_kernel(const float* __restrict_
   ss = warp_sum(ss);
   const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
 #pragma unroll
-  for (int k = 0; k < 8; ++k) out[(long long)(lane + 32 * k) * n + warp] = v[k] * inv;
+  for (int k = 0; k < 8; ++k) out[(lane + 32 * k) * stride] = v[k] * inv;
+}
+
+// one image: keypoints [n, 2] -> out [256, n]
+__global__ void __launch_bounds__(256) sp_sample_kernel(const float* __restrict__ dense, const float* __restrict__ kpts,
+                                                        float* __restrict__ out, int n, int h, int w) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= n) return;
+  sp_sample_point(dense, kpts + 2 * warp, h, w, lane, out + warp, n);
+}
+
+// a batch: dense [B, h, w, 256], keypoints [B, K, 2], counts [B] -> out [B, 256, K]; columns at or past counts[b] are
+// zero
+__global__ void __launch_bounds__(256) sp_sample_batch_kernel(const float* __restrict__ dense,
+                                                              const float* __restrict__ kpts,
+                                                              const int* __restrict__ counts, float* __restrict__ out,
+                                                              int B, int K, int h, int w) {
+  const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (warp >= (long long)B * K) return;
+  const int b = (int)(warp / K), i = (int)(warp % K);
+  float* o = out + (long long)b * 256 * K + i;
+  if (i >= counts[b]) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) o[(long long)(lane + 32 * k) * K] = 0.f;
+    return;
+  }
+  sp_sample_point(dense + (long long)b * h * w * 256, kpts + 2 * warp, h, w, lane, o, K);
+}
+
+// ---- batched keypoint selection (superpoint.py:181-189 without the host round trips) ----------------------------------
+// One CTA per image scans its score map [Hs, Ws] (Hs, Ws multiples of 8, so a float4 never crosses a row).  Candidates
+// are the pixels with score > threshold inside the border (remove_borders).  With at most K candidates they are written
+// in raster order, which is what torch.nonzero + top_k_keypoints gives when k >= len.  With more, an MSB-first radix
+// select over the order-preserving 32-bit keys of the scores (four 8-bit digits, one pass over the map each) finds the
+// K-th largest key T and how many keys equal to T are taken; those are the first ones in raster order (the tie rule:
+// lower y * Ws + x first).  The K chosen (key, index) pairs are bitonic-sorted in shared memory: descending score,
+// ties by raster index.  Candidates are sparse after NMS, so the shared-memory atomics of the histograms are few; the
+// cost is the five reads of the map, spread over B CTAs.
+constexpr int SEL_THREADS = 1024;
+constexpr int SEL_WARPS = SEL_THREADS / 32;
+
+__device__ __forceinline__ unsigned sp_order_key(float s) {   // a > b as floats <=> key(a) > key(b) as unsigned
+  const unsigned u = __float_as_uint(s);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// exclusive block-wide prefix sum of v; *total = sum over the block.  Every thread of the block must call it.
+__device__ __forceinline__ int sp_block_scan(int v, int* s_warp, int* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) s_warp[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    int t = s_warp[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, t, o);
+      if (lane >= o) t += y;
+    }
+    s_warp[lane] = t;
+  }
+  __syncthreads();
+  const int excl = x - v + (wid ? s_warp[wid - 1] : 0);
+  *total = s_warp[SEL_WARPS - 1];
+  __syncthreads();                                     // s_warp is reused by the next call
+  return excl;
+}
+
+// grid = B, block = SEL_THREADS, dynamic shared memory = P * 8 bytes, P = the power of two >= K
+__global__ void __launch_bounds__(SEL_THREADS) sp_select_kernel(const float* __restrict__ scores, int Hs, int Ws,
+                                                                float thr, int border, int K, float* __restrict__ kpts,
+                                                                float* __restrict__ out_scores, int* __restrict__ counts) {
+  extern __shared__ unsigned long long s_sel[];        // (key << 32) | ~index: descending order = the output order
+  __shared__ int s_hist[256];
+  __shared__ int s_warp[SEL_WARPS];
+  __shared__ unsigned s_prefix;
+  __shared__ int s_krem;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int n = Hs * Ws, n4 = n / 4;
+  const float* map = scores + (long long)b * n;
+  const float4* map4 = reinterpret_cast<const float4*>(map);
+  float* kp_out = kpts + (long long)b * K * 2;
+  float* sc_out = out_scores + (long long)b * K;
+  auto candidate = [&](int idx, float s) {
+    const int y = idx / Ws, x = idx - y * Ws;
+    return s > thr && y >= border && y < Hs - border && x >= border && x < Ws - border;
+  };
+
+  // radix select: after pass p, prefix holds the top 8 (p + 1) bits of T and krem the rank of T among the keys that
+  // share them
+  unsigned prefix = 0;
+  int krem = K, total = 0;
+  for (int pass = 0; pass < 4; ++pass) {
+    const int shift = 24 - 8 * pass;
+    for (int i = tid; i < 256; i += SEL_THREADS) s_hist[i] = 0;
+    __syncthreads();
+    for (int i4 = tid; i4 < n4; i4 += SEL_THREADS) {
+      const float4 v4 = map4[i4];
+      const float v[4] = {v4.x, v4.y, v4.z, v4.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (!candidate(4 * i4 + j, v[j])) continue;
+        const unsigned key = sp_order_key(v[j]);
+        if (pass == 0 || (key ^ prefix) >> (shift + 8) == 0) atomicAdd(&s_hist[(key >> shift) & 255], 1);
+      }
+    }
+    __syncthreads();
+    const int c = tid < 256 ? s_hist[255 - tid] : 0;   // bins from the largest digit down
+    int sum;
+    const int above = sp_block_scan(c, s_warp, &sum);
+    if (pass == 0) {
+      total = sum;
+      if (total <= K) break;                           // uniform: every thread has the same sum
+    }
+    if (tid < 256 && above < krem && above + c >= krem) {
+      s_prefix = prefix | ((unsigned)(255 - tid) << shift);
+      s_krem = krem - above;
+    }
+    __syncthreads();
+    prefix = s_prefix;
+    krem = s_krem;
+    __syncthreads();
+  }
+  if (tid == 0) counts[b] = total;
+
+  if (total <= K) {
+    // every candidate, raster order, straight to the outputs; zeros past the count
+    int base = 0;
+    for (int t0 = 0; t0 < n4; t0 += SEL_THREADS) {
+      const int i4 = t0 + tid;
+      float v[4] = {0.f, 0.f, 0.f, 0.f};
+      bool take[4] = {false, false, false, false};
+      int mine = 0;
+      if (i4 < n4) {
+        const float4 v4 = map4[i4];
+        v[0] = v4.x; v[1] = v4.y; v[2] = v4.z; v[3] = v4.w;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { take[j] = candidate(4 * i4 + j, v[j]); mine += take[j]; }
+      }
+      int tile;
+      int pos = base + sp_block_scan(mine, s_warp, &tile);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (!take[j]) continue;
+        const int idx = 4 * i4 + j, y = idx / Ws;
+        kp_out[2 * pos] = (float)(idx - y * Ws);
+        kp_out[2 * pos + 1] = (float)y;
+        sc_out[pos] = v[j];
+        ++pos;
+      }
+      base += tile;
+    }
+    for (int i = total + tid; i < K; i += SEL_THREADS) {
+      kp_out[2 * i] = 0.f;
+      kp_out[2 * i + 1] = 0.f;
+      sc_out[i] = 0.f;
+    }
+    return;
+  }
+
+  // more than K candidates: the keys above T, and the first krem keys equal to T in raster order
+  const unsigned T = prefix;
+  int base = 0, eq_base = 0;
+  for (int t0 = 0; t0 < n4; t0 += SEL_THREADS) {
+    const int i4 = t0 + tid;
+    unsigned key[4] = {0u, 0u, 0u, 0u};
+    bool cand[4] = {false, false, false, false};
+    int n_eq = 0;
+    if (i4 < n4) {
+      const float4 v4 = map4[i4];
+      const float v[4] = {v4.x, v4.y, v4.z, v4.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        cand[j] = candidate(4 * i4 + j, v[j]);
+        key[j] = sp_order_key(v[j]);
+        n_eq += cand[j] && key[j] == T;
+      }
+    }
+    int eq_tile;
+    int eq_rank = eq_base + sp_block_scan(n_eq, s_warp, &eq_tile);
+    bool take[4];
+    int mine = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      take[j] = cand[j] && (key[j] > T || (key[j] == T && eq_rank < krem));
+      eq_rank += cand[j] && key[j] == T;
+      mine += take[j];
+    }
+    int tile;
+    int pos = base + sp_block_scan(mine, s_warp, &tile);
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (take[j]) s_sel[pos++] = ((unsigned long long)key[j] << 32) | (unsigned)~(unsigned)(4 * i4 + j);
+    base += tile;
+    eq_base += eq_tile;
+  }
+  int P = 1;
+  while (P < K) P <<= 1;
+  for (int i = K + tid; i < P; i += SEL_THREADS) s_sel[i] = 0ull;   // below every real entry: no finite score has key 0
+  __syncthreads();
+  for (int k = 2; k <= P; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = tid; i < P; i += SEL_THREADS) {
+        const int l = i ^ j;
+        if (l > i) {
+          const unsigned long long a = s_sel[i], c = s_sel[l];
+          if ((i & k) == 0 ? a < c : a > c) { s_sel[i] = c; s_sel[l] = a; }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  for (int i = tid; i < K; i += SEL_THREADS) {
+    const int idx = (int)~(unsigned)(s_sel[i] & 0xffffffffull), y = idx / Ws;
+    kp_out[2 * i] = (float)(idx - y * Ws);
+    kp_out[2 * i + 1] = (float)y;
+    sc_out[i] = map[idx];
+  }
 }
 
 int conv3x3(const float* in, const float* w, const float* b, float* out, int B, int H, int W, int Cin, int Cout, int relu,
@@ -364,6 +588,45 @@ int mvm_superpoint_sample(const float* dense_desc, const float* keypoints, int n
   if (n == 0) return MVM_OK;
   MvmProfScope prof__(MVM_TAG_MISC, s);
   sp_sample_kernel<<<(n * 32 + 255) / 256, 256, 0, s>>>(dense_desc, keypoints, descriptors, n, h, w);
+  MVM_CHECK_LAUNCH();
+  return MVM_OK;
+}
+
+int mvm_superpoint_select(const float* scores_nms, int batch, int height, int width, float keypoint_threshold,
+                          int remove_borders, int max_keypoints, float* keypoints, float* scores, int* counts,
+                          void* stream_) {
+  cudaStream_t s = (cudaStream_t)stream_;
+  MVM_REQUIRE(scores_nms && keypoints && scores && counts);
+  MVM_REQUIRE(((uintptr_t)scores_nms & 15) == 0);                                     // read as float4
+  MVM_REQUIRE(batch >= 1 && height >= 8 && width >= 8 && height % 8 == 0 && width % 8 == 0);
+  MVM_REQUIRE((long long)height * width <= 0x7fffffffLL && batch <= 65535);
+  MVM_REQUIRE(remove_borders >= 0 && keypoint_threshold == keypoint_threshold);        // not NaN
+  MVM_REQUIRE(max_keypoints >= 1 && max_keypoints <= MVM_SUPERPOINT_MAX_SELECT &&
+              (long long)max_keypoints <= (long long)height * width);
+  MvmProfScope prof__(MVM_TAG_MISC, s);
+  int P = 1;
+  while (P < max_keypoints) P <<= 1;
+  const int smem = P * (int)sizeof(unsigned long long);
+  mvm_once_per_device(MVM_ONCE_SP_SELECT, [&] {
+    cudaFuncSetAttribute(sp_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         MVM_SUPERPOINT_MAX_SELECT * (int)sizeof(unsigned long long));
+  });
+  sp_select_kernel<<<batch, SEL_THREADS, smem, s>>>(scores_nms, height, width, keypoint_threshold, remove_borders,
+                                                    max_keypoints, keypoints, scores, counts);
+  MVM_CHECK_LAUNCH();
+  return MVM_OK;
+}
+
+int mvm_superpoint_sample_batch(const float* dense_desc, const float* keypoints, const int* counts, int batch,
+                                int max_keypoints, int h, int w, float* descriptors, void* stream_) {
+  cudaStream_t s = (cudaStream_t)stream_;
+  MVM_REQUIRE(dense_desc && keypoints && counts && descriptors);
+  MVM_REQUIRE(batch >= 1 && max_keypoints >= 1 && h >= 1 && w >= 1);
+  const long long warps = (long long)batch * max_keypoints;
+  MVM_REQUIRE(warps * 32 / 256 < 0x7fffffffLL);
+  MvmProfScope prof__(MVM_TAG_MISC, s);
+  sp_sample_batch_kernel<<<(int)((warps * 32 + 255) / 256), 256, 0, s>>>(dense_desc, keypoints, counts, descriptors,
+                                                                         batch, max_keypoints, h, w);
   MVM_CHECK_LAUNCH();
   return MVM_OK;
 }

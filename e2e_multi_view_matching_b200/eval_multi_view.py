@@ -5,7 +5,15 @@ trained checkpoint; neither exists offline, so tuples are synthetic scenes
 (synthetic.make_scene_tuple_inputs) and weights are either a reference checkpoint given with --ckpt
 (helpers.load_ckpt format: {'model': state_dict with 'module.' prefix}) or seeded random weights.
 
+With --images the tuples are image-in, as in the reference: the scene is rendered into every view
+(synthetic.render_tuple_images) and SuperPoint (seeded weights, or a superpoint_v1.pth-style state dict given with
+--superpoint_weights; max_keypoints, keypoint_threshold, nms_radius and remove_borders as eval_multi_view.py:125-141)
+finds the keypoints on the device before the matcher (run_super_point, eval_multi_view.py:157), one tuple per batch as
+the reference's test loader (batch_size=1), so every view keeps its own keypoint count.  Without it, the matcher gets
+the synthetic keypoints directly.
+
     python -m e2e_multi_view_matching_b200.eval_multi_view --n_tuples 16 --out result.json
+    python -m e2e_multi_view_matching_b200.eval_multi_view --images --n_tuples 16 --out result.json
 """
 import argparse
 import json
@@ -14,8 +22,9 @@ import numpy as np
 import torch
 
 from .models.multi_view_matcher import MultiViewMatcher
+from .models.superpoint import SuperPoint
 from .pipeline import MultiViewPipeline, pose_auc
-from .synthetic import make_state_dict, make_scene_tuple_inputs
+from .synthetic import make_state_dict, make_scene_tuple_inputs, make_superpoint_state_dict, render_tuple_images
 
 
 def write_result(pose_errors, file):
@@ -41,6 +50,11 @@ def main(argv=None):
     ap.add_argument('--seed', type=int, default=0)
     ap.add_argument('--math_mode', type=int, default=3)
     ap.add_argument('--out', default=None)
+    ap.add_argument('--images', action='store_true', help='render the tuples and run SuperPoint on them')
+    ap.add_argument('--superpoint_weights', default=None)
+    ap.add_argument('--keypoint_threshold', type=float, default=0.005)
+    ap.add_argument('--nms_radius', type=int, default=4)
+    ap.add_argument('--remove_borders', type=int, default=4)
     opt = ap.parse_args(argv)
     import e2e_multi_view_matching_b200 as pkg
     pkg.set_math_mode(opt.math_mode)
@@ -62,15 +76,30 @@ def main(argv=None):
         sd = make_state_dict(len(layers), seed=opt.seed, final_proj_gain=12.0, conf_head='score')
         matcher.load_state_dict({k: torch.from_numpy(np.asarray(v)) for k, v in sd.items()})
     matcher = matcher.cuda()
-    pipe = MultiViewPipeline(matcher)
+    superpoint = None
+    if opt.images:
+        superpoint = SuperPoint({'max_keypoints': opt.max_keypoints, 'keypoint_threshold': opt.keypoint_threshold,
+                                 'nms_radius': opt.nms_radius, 'remove_borders': opt.remove_borders,
+                                 'weights': opt.superpoint_weights}).eval()
+        if not opt.superpoint_weights:
+            superpoint.load_state_dict({k: torch.from_numpy(v) for k, v in make_superpoint_state_dict(opt.seed).items()})
+        superpoint = superpoint.cuda()
+        opt.batch = 1
+    pipe = MultiViewPipeline(matcher, superpoint=superpoint)
     pose_errors = [[], [], []]
     with torch.no_grad():
         for start in range(0, opt.n_tuples, opt.batch):
             b = min(opt.batch, opt.n_tuples - start)
-            data = make_scene_tuple_inputs(1000 + start, opt.tuple_size, opt.max_keypoints, batch=b)
-            data = {k: (torch.from_numpy(v).cuda() if isinstance(v, np.ndarray) and not k.startswith('image')
-                        else (torch.empty(v.shape, device='meta') if isinstance(v, np.ndarray) else v))
-                    for k, v in data.items()}
+            if opt.images:
+                data = render_tuple_images(make_scene_tuple_inputs(1000 + start, opt.tuple_size, opt.max_keypoints,
+                                                                   batch=b, noise_px=0.0), seed=1000 + start)
+                data = {k: (torch.from_numpy(v).cuda() if isinstance(v, np.ndarray) else v) for k, v in data.items()
+                        if not k.startswith(('keypoints', 'scores', 'descriptors'))}
+            else:
+                data = make_scene_tuple_inputs(1000 + start, opt.tuple_size, opt.max_keypoints, batch=b)
+                data = {k: (torch.from_numpy(v).cuda() if isinstance(v, np.ndarray) and not k.startswith('image')
+                            else (torch.empty(v.shape, device='meta') if isinstance(v, np.ndarray) else v))
+                        for k, v in data.items()}
             _, pose = pipe(data)
             for e in MultiViewPipeline.pair_errors(data, pose, opt.tuple_size):
                 for i in range(3):

@@ -1,8 +1,9 @@
 """SuperPoint with the reference's constructor, config keys, state-dict keys and forward(data) -> dict contract
 (models/models/superpoint.py:102-229), computing in libmvm_b200.so: the VGG encoder, both heads, the three-round
 non-maximum suppression and the descriptor sampling are CUDA kernels (csrc/superpoint.cu); the nn.Conv2d modules below
-only own the parameters under the reference's key names.  What stays in torch is index book-keeping on the NMS output
-(nonzero / border mask / top-k), as in the reference.  No CPU fallback.
+only own the parameters under the reference's key names.  In forward, what stays in torch is index book-keeping on the
+NMS output (nonzero / border mask / top-k), as in the reference; forward_batch does that selection on the device too,
+for a whole batch in one launch.  No CPU fallback.
 
 `weights`: path of a `superpoint_v1.pth`-style state dict, or None to keep the random initialisation (then load one with
 load_state_dict); the reference hard-codes the path next to its source file, which does not exist here."""
@@ -152,3 +153,48 @@ class SuperPoint(nn.Module):
                     all_scores.append(sc)
                     all_descriptors.append(desc)
         return {'keypoints': all_keypoints, 'scores': all_scores, 'descriptors': all_descriptors}
+
+    def forward_batch(self, images):
+        """forward for one batch of images [B,1,H,W] whose results are used as stacked tensors (run_super_point): needs
+        max_keypoints = K > 0 and returns {'keypoints' [B,K,2] (x, y), 'scores' [B,K], 'descriptors' [B,256,K],
+        'counts' [B] int32 = valid entries per image}.  Selection and sampling are one launch each for the batch
+        (mvm_superpoint_select / mvm_superpoint_sample_batch) and do not synchronise with the host.  Entries at or past
+        an image's count are zero.  Per image the result is forward's, bit for bit, except for the order among equal
+        scores: torch.topk leaves it open, here the lower raster index comes first (also at the K-th score).
+
+        With fill_with_random_keypoints the [B] counts are read once (one synchronisation per batch) and every short
+        image is filled with the same torch.randint calls, in the same order, as forward makes, so the fill draws the
+        same keypoints from the same generator state; counts are then K."""
+        K = self.config['max_keypoints']
+        if K < 0:
+            raise ValueError('forward_batch needs "max_keypoints" > 0 (fixed-size outputs); use forward')
+        lib = _lib.lib()
+        with torch.no_grad():
+            scores_map, dense = self.dense(images)
+            B, H, Wd = scores_map.shape
+            h, w = H // 8, Wd // 8
+            dev = scores_map.device
+            kxy = torch.empty(B, K, 2, dtype=torch.float32, device=dev)
+            sc = torch.empty(B, K, dtype=torch.float32, device=dev)
+            counts = torch.empty(B, dtype=torch.int32, device=dev)
+            with torch.cuda.device(dev):
+                rc = lib.mvm_superpoint_select(_lib.ptr(scores_map), B, H, Wd, float(self.config['keypoint_threshold']),
+                                               int(self.config['remove_borders']), K, _lib.ptr(kxy), _lib.ptr(sc),
+                                               _lib.ptr(counts), _lib.stream_ptr())
+            _lib.check(rc, 'mvm_superpoint_select')
+            counts.clamp_(max=K)
+            if self.config['fill_with_random_keypoints']:
+                border = self.config['remove_borders']
+                for bi, n in enumerate(counts.tolist()):
+                    if n < K:
+                        add_n = K - n
+                        add_k = torch.cat((torch.randint(border, h * 8 - border, (add_n, 1), device=dev),
+                                           torch.randint(border, w * 8 - border, (add_n, 1), device=dev)), 1)
+                        kxy[bi, n:] = torch.flip(add_k, [1]).float()
+                counts.fill_(K)
+            desc = torch.empty(B, 256, K, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                rc = lib.mvm_superpoint_sample_batch(_lib.ptr(dense), _lib.ptr(kxy), _lib.ptr(counts), B, K, h, w,
+                                                     _lib.ptr(desc), _lib.stream_ptr())
+            _lib.check(rc, 'mvm_superpoint_sample_batch')
+        return {'keypoints': kxy, 'scores': sc, 'descriptors': desc, 'counts': counts}

@@ -5,8 +5,11 @@
   PairPipeline.__call__       ==  eval_pairs.py:208-267 for the w8pt / w8pt_ba / ransac / ransac_ba modes
 
 Inputs are the reference's `data` dicts (keypoints{i}, scores{i}, descriptors{i}, image{i}, intr{i},
-ids); there is no numpy hop between matcher and pose, no subprocess and no CSV file.
+ids; MultiViewPipeline with a SuperPoint front-end also takes image{i} without keypoints); there is no numpy hop
+between matcher and pose, no subprocess and no CSV file.
 """
+import types
+
 import numpy as np
 import torch
 
@@ -41,19 +44,36 @@ def pose_auc(errors, thresholds):
 
 
 class MultiViewPipeline:
-    """matcher (multi_frame_matching=True) + multi-view pose stage for batches of tuples."""
+    """[SuperPoint +] matcher (multi_frame_matching=True) + multi-view pose stage for batches of tuples."""
 
-    def __init__(self, matcher: MultiViewMatcher, conf_thresh=0.0):
+    def __init__(self, matcher: MultiViewMatcher, conf_thresh=0.0, superpoint=None):
         assert matcher.config['multi_frame_matching'] and matcher.config['conf_mlp']
         self.matcher = matcher
+        self.superpoint = superpoint
         self.pose = MultiViewPoseEngine(conf_thresh=conf_thresh)
 
     def __call__(self, data, global_ba=True):
-        """-> (matcher result, pose).  Views without keypoints are skipped by the matcher (multi_view_matcher.py:
-        155-162), so the pose stage works on view SLOTS: pose['view_ids'][s] is the id (in `data`) of slot s, the
-        extrinsics / pair tensors are indexed by slot.  pose is None when fewer than two views have keypoints
-        (nothing to estimate: the reference's "cannot compute pose" case)."""
+        """-> (matcher result, pose).  When `data` has no keypoints0, the `superpoint` front-end runs on image{i} first
+        (run_super_point, as eval_multi_view.py:157 does; views of one image size run as one batch) and the result
+        also carries its keypoints{i} / scores{i} / descriptors{i}; the caller's dict is left as it is.  Views without
+        keypoints are skipped by the matcher (multi_view_matcher.py:155-162), so the pose stage works on view SLOTS:
+        pose['view_ids'][s] is the id (in `data`) of slot s, the extrinsics / pair tensors are indexed by slot.  pose
+        is None when fewer than two views have keypoints (nothing to estimate: the reference's "cannot compute pose"
+        case)."""
+        features = {}
+        if 'keypoints0' not in data:
+            if self.superpoint is None:
+                raise ValueError('keypoints0 missing and no SuperPoint front-end given')
+            from .training import run_super_point
+            views = ['image%d' % i for i in range(len(data['ids']))]
+            batch = data['image0'].shape[0]
+            data = dict(data)
+            before = set(data)
+            run_super_point(types.SimpleNamespace(batch_size=batch), data, self.superpoint,
+                            merge=len({tuple(data[k].shape) for k in views}) == 1)
+            features = {k: data[k] for k in set(data) - before}
         result = self.matcher(data)
+        result.update(features)
         state = self.matcher._engine.last
         if state is None:
             return result, None

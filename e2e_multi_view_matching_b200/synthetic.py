@@ -232,6 +232,32 @@ def make_scene_tuple_inputs(seed, n_views=5, n_kpts=1024, batch=1, width=640, he
     return out
 
 
+def render_tuple_images(data, seed=0, blob_sigma=2.0):
+    """Render image{i} [B,1,H,W] in [0,1] for a make_scene_tuple_inputs tuple (best made with noise_px=0): every
+    landmark a view sees is drawn as a Gaussian blob of radius ~blob_sigma px at its projection keypoints{i}, with a
+    contrast of its own (bright or dark) on a mid-grey background, so that all views show the same scene points.  The
+    image-in input of the multi-view evaluation; replaces the zero images in `data` in place and returns it."""
+    rng = np.random.default_rng(seed)
+    n_land = max(int(data['landmark%d' % i].max()) for i in data['ids']) + 1
+    contrast = rng.uniform(0.4, 1.0, n_land) * rng.choice([-1.0, 1.0], n_land)
+    r = int(np.ceil(3 * blob_sigma))
+    g = np.exp(-np.arange(-r, r + 1) ** 2 / (2 * blob_sigma ** 2))         # peak 1: a lone blob reaches its contrast
+    for i in data['ids']:
+        B, _, H, W = data['image%d' % i].shape
+        out = np.zeros((B, 1, H, W), np.float32)
+        for b in range(B):
+            acc = np.zeros((H, W))
+            kp = data['keypoints%d' % i][b]
+            x = np.clip(np.rint(kp[:, 0]).astype(np.int64), 0, W - 1)
+            y = np.clip(np.rint(kp[:, 1]).astype(np.int64), 0, H - 1)
+            np.add.at(acc, (y, x), contrast[data['landmark%d' % i][b]])
+            acc = np.apply_along_axis(lambda row: np.convolve(row, g, mode='same'), 1, acc)
+            acc = np.apply_along_axis(lambda col: np.convolve(col, g, mode='same'), 0, acc)
+            out[b, 0] = np.clip(0.5 + 0.5 * acc, 0.0, 1.0)
+        data['image%d' % i] = out
+    return data
+
+
 def make_superpoint_state_dict(seed=0, logit_gain=3.0):
     """Seeded SuperPoint weights with the reference's keys/shapes (models/models/superpoint.py:120-137): He-uniform
     convolutions; the detector logits are scaled by `logit_gain` so that the 65-way softmax has peaks."""

@@ -1,6 +1,10 @@
 """Training-side consumers of the matcher output -- SURVEY.md §8 f-2 / a20 (BASELINE cfg5).
 
 Built:
+  * run_super_point (helpers.py:83-96): SuperPoint on the images of a tuple batch, merged batches through
+    SuperPoint.forward_batch (keypoint selection and descriptor sampling on the device, one launch each, one dense pass
+    whether or not every image reaches max_keypoints);
+    train_step / validation_step call it when the batch has images and no keypoints;
   * compute_match_loss (helpers.py:228-241) as an autograd.Function on CUDA kernels (csrc/train_loss.cu), forward
     and backward;
   * combine_losses (train.py:36-40);
@@ -129,6 +133,55 @@ def compute_gt_matches_of_image_pair(kpts0, kpts1, K0, K1, T0to1, depth0, depth1
     return indices, weights
 
 
+def run_super_point(opt, data, super_point, merge=True):
+    """helpers.py:83-96: SuperPoint on image{m} of every view m of the tuple, results as data['keypoints' + m],
+    data['scores' + m], data['descriptors' + m] ([B,N,2], [B,N], [B,256,N]).  With merge the T views' [B,1,H,W] batches
+    run as one through SuperPoint.forward_batch (when 0 < max_keypoints <= MVM_SUPERPOINT_MAX_SELECT and max_keypoints
+    is at most the score map's pixel count).  When every image ends with max_keypoints keypoints (always so with
+    fill_with_random_keypoints) its [T*B, ...] tensors are viewed as [T, B, ...]; otherwise each image's valid entries
+    become the per-image lists forward would give (bitwise; among equal scores at the cut, the selection's tie rule)
+    without a second dense pass.  merge=False and the other configurations go through SuperPoint.forward.  The lists
+    are stacked as the reference does (batch size 1: each image's tensors with a leading 1)."""
+    curr_tuple_size = len(data["ids"])
+    images = [data["image" + str(i)].cuda() for i in range(curr_tuple_size)]
+    if merge:
+        images = [torch.cat(images, 0)]
+    k_max = super_point.config['max_keypoints']
+    map_px = (images[0].shape[-2] // 8 * 8) * (images[0].shape[-1] // 8 * 8)
+    with torch.no_grad():
+        if merge and 0 < k_max <= min(_lib.MVM_SUPERPOINT_MAX_SELECT, map_px):
+            out = super_point.forward_batch(images[0])
+            counts = out['counts'].tolist() if not super_point.config['fill_with_random_keypoints'] else None
+            if counts is None or all(n == k_max for n in counts):
+                for k in ('keypoints', 'scores', 'descriptors'):
+                    res = out[k].view(curr_tuple_size, opt.batch_size, *out[k].shape[1:])
+                    for m in range(curr_tuple_size):
+                        data[k + str(m)] = res[m]
+                return
+            pred = {'keypoints': [out['keypoints'][b, :n] for b, n in enumerate(counts)],
+                    'scores': [out['scores'][b, :n] for b, n in enumerate(counts)],
+                    'descriptors': [out['descriptors'][b, :, :n].contiguous() for b, n in enumerate(counts)]}
+        else:
+            pred = super_point({"image": images})
+        for k, v in pred.items():
+            if len(v) != curr_tuple_size:  # batch size > 1
+                res = torch.stack(v)
+                res = res.view(curr_tuple_size, opt.batch_size, *res.shape[1:])
+            else:  # batch size 1
+                res = [v_i.unsqueeze(0) for v_i in v]
+            for m in range(curr_tuple_size):
+                data[k + str(m)] = res[m]
+
+
+def _images_in(data, super_point):
+    """True when the batch carries images and no keypoints yet: SuperPoint runs first (train.py:409)."""
+    if "image0" not in data or "keypoints0" in data:
+        return False
+    if super_point is None:
+        raise ValueError('the batch has images and no keypoints: pass super_point= to run SuperPoint on them')
+    return True
+
+
 def compute_gt_matches(opt, data):
     """helpers.py:215-226: gt_indices_k_m / gt_weights_k_m for every pair k < m of the tuple; pops the depth maps."""
     curr_tuple_size = len(data["ids"])
@@ -171,11 +224,14 @@ def run_matcher(opt, data, matcher):
     return losses, result
 
 
-def validation_step(opt, data, matcher, n_pairs, pose_match_ratio, process_group=None):
-    """One batch of Trainer.validate (train.py:89-106) after SuperPoint: ground-truth matches when the batch still
-    carries depth maps, run_matcher, combine_losses; the scalar validation loss is all-reduced over the ranks
-    (mean) when torch.distributed is initialised.  -> (val_loss tensor [1], losses dict)."""
+def validation_step(opt, data, matcher, n_pairs, pose_match_ratio, process_group=None, super_point=None):
+    """One batch of Trainer.validate (train.py:89-106): run_super_point when the batch carries images and no keypoints
+    (then `super_point` is required), ground-truth matches when it still carries depth maps, run_matcher,
+    combine_losses; the scalar validation loss is all-reduced over the ranks (mean) when torch.distributed is
+    initialised.  -> (val_loss tensor [1], losses dict)."""
     with torch.no_grad():
+        if _images_in(data, super_point):
+            run_super_point(opt, data, super_point)
         if "depth0" in data:
             compute_gt_matches(opt, data)
         losses, _ = run_matcher(opt, data, matcher)
@@ -187,14 +243,17 @@ def validation_step(opt, data, matcher, n_pairs, pose_match_ratio, process_group
     return val_loss, losses
 
 
-def train_step(opt, data, matcher, optimizer, n_pairs, pose_match_ratio=0.0, grad_clip=-1.0):
-    """One iteration of the training loop after SuperPoint (train.py:409-426), stage 1 (match loss): ground-truth matches
-    when the batch still carries depth maps, run_matcher in train mode, combine_losses, backward through the kernels,
-    gradient averaging over the ranks when torch.distributed is initialised (DistributedDataParallel's all-reduce in the
-    reference), optional value clipping, optimiser step.  -> (train_loss tensor, losses dict)."""
+def train_step(opt, data, matcher, optimizer, n_pairs, pose_match_ratio=0.0, grad_clip=-1.0, super_point=None):
+    """One iteration of the training loop (train.py:409-426), stage 1 (match loss): run_super_point when the batch
+    carries images and no keypoints (then `super_point` is required), ground-truth matches when it still carries depth
+    maps, run_matcher in train mode, combine_losses, backward through the kernels, gradient averaging over the ranks
+    when torch.distributed is initialised (DistributedDataParallel's all-reduce in the reference), optional value
+    clipping, optimiser step.  -> (train_loss tensor, losses dict)."""
     if getattr(opt, 'pose_loss', False):
         raise NotImplementedError('stage 2 (--pose_loss) needs the gradients of the pose stage, which are not built')
     from . import sharding
+    if _images_in(data, super_point):
+        run_super_point(opt, data, super_point)
     if "depth0" in data:
         with torch.no_grad():
             compute_gt_matches(opt, data)

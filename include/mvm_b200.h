@@ -446,6 +446,28 @@ int mvm_superpoint_dense(const mvm_superpoint_weights* w, const float* image, in
 int mvm_superpoint_sample(const float* dense_desc, const float* keypoints, int n, int h, int w, float* descriptors,
                           void* stream);
 
+/* Largest max_keypoints mvm_superpoint_select takes: the chosen keypoints are sorted in shared memory. */
+#define MVM_SUPERPOINT_MAX_SELECT 16384
+
+/* Keypoint selection of SuperPoint.forward (:181-189) for a whole batch in one launch, without host synchronisation:
+ * scores_nms [batch, height, width] as mvm_superpoint_dense writes it (height, width multiples of 8) -> counts [batch]
+ * int32 = the number of candidates (score > keypoint_threshold, at least remove_borders pixels inside every edge), and
+ * keypoints [batch, max_keypoints, 2] (x, y as float) with scores [batch, max_keypoints]:
+ *   - counts[b] <= max_keypoints: every candidate in raster order (what nonzero + top_k_keypoints gives), zeros after;
+ *   - counts[b] >  max_keypoints: the max_keypoints largest scores in descending order (top_k_keypoints).  Tie rule:
+ *     among equal scores the lower raster index y * width + x comes first, also when the tie straddles the cut.
+ * 1 <= max_keypoints <= min(height * width, MVM_SUPERPOINT_MAX_SELECT); scores_nms 16-byte aligned. */
+int mvm_superpoint_select(const float* scores_nms, int batch, int height, int width, float keypoint_threshold,
+                          int remove_borders, int max_keypoints, float* keypoints, float* scores, int* counts,
+                          void* stream);
+
+/* mvm_superpoint_sample for a batch in one launch: dense_desc [batch, h, w, 256], keypoints [batch, max_keypoints, 2],
+ * counts [batch] -> descriptors [batch, 256, max_keypoints], the matcher's layout.  The same device code as
+ * mvm_superpoint_sample, so the descriptors are bitwise those of the per-image call; columns at or past counts[b] are
+ * zero. */
+int mvm_superpoint_sample_batch(const float* dense_desc, const float* keypoints, const int* counts, int batch,
+                                int max_keypoints, int h, int w, float* descriptors, void* stream);
+
 /* ---- training path (SURVEY.md §8 a20 / f-2): losses, ground-truth matches, train-mode BatchNorm, backward kernels ---- */
 
 /* compute_match_loss (helpers.py:228-241): weighted NLL of the ground-truth assignment on the log-couplings.
