@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(_HERE, 'libmvm_b200.so')
 MVM_MAX_LAYERS = 64
 MVM_MAX_VIEWS = 8
 MVM_SUPERPOINT_MAX_SELECT = 16384
+MVM_CONF_MAX_PAIRS = 28
 
 _fp = C.c_void_p  # device pointers travel as integers
 
@@ -90,6 +91,14 @@ def lib():
     L.mvm_batchnorm_train_backward.argtypes = [_fp, _fp, _fp, I, I, I, I, I, I, I, _fp, _fp, I, _fp, _fp, I, _fp, _fp]
     L.mvm_colsum.restype = I
     L.mvm_colsum.argtypes = [_fp, I, I, I, _fp, I, _fp, _fp]
+    L.mvm_conf_backward_ws_doubles.restype = C.c_size_t
+    L.mvm_conf_backward_ws_doubles.argtypes = [I]
+    L.mvm_debug_set_conf_i0_check.restype = None
+    L.mvm_debug_set_conf_i0_check.argtypes = [I]
+    L.mvm_conf_tail_backward.restype = I
+    L.mvm_conf_tail_backward.argtypes = [_fp, _fp, _fp, _fp, I, _fp, _fp, _fp, _fp, C.c_size_t, _fp]
+    L.mvm_conf_gather_backward.restype = I
+    L.mvm_conf_gather_backward.argtypes = [_fp] * 5 + [I] * 5 + [C.POINTER(I), C.POINTER(I)] + [_fp] * 4 + [C.c_size_t, _fp]
     L.mvm_transpose_split.restype = I
     L.mvm_transpose_split.argtypes = [_fp, I, I, I, _fp, _fp, _fp, C.c_longlong, _fp]
     L.mvm_attention_backward.restype = I

@@ -170,6 +170,9 @@ class MultiViewMatcher(nn.Module):
         'multi_frame_matching': True,
         'full_output': False,
         'conf_mlp': True,
+        # not a reference key: in train mode with full_output, conf_scores_* carry a graph into the confidence head and
+        # the matcher (training.run_matcher sets it with pose_loss); the eval path does not read it
+        'conf_grad': False,
     }
 
     def __init__(self, config):

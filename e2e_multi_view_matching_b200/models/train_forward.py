@@ -12,9 +12,16 @@ statistics cannot be folded, so the train branch sequences the stage kernels fro
 The whole matcher is ONE autograd.Function (`MatcherTrainFn`): its inputs are the module's parameters, its outputs the
 coupling matrices, so `loss.backward()`, torch optimisers and DistributedDataParallel's gradient hooks work unchanged.
 
-Not differentiable here (stated, not hidden): `matching_scores*` / `conf_scores_*` -- the pose-loss half of cfg5
-(gradients through the weighted eight-point, the two-view BA and the ConfidenceMLP) is not built; with `full_output` those
-tensors are returned without a graph."""
+The confidence head's graph is opt-in, through the matcher config key `conf_grad` (default False; training.run_matcher
+sets it to opt.pose_loss, like `full_output`).  With `full_output` and `conf_grad` in train mode under autograd, the
+forward keeps the head's state of every pair (its inputs m0, m1g and the score input, the pre- and post-BatchNorm
+activations and statistics, h = out_f + out_c, the sigmoid output, the matches) and `conf_scores_*` are differentiable
+outputs beside `scores_*`.  Their gradient runs back through the head (`mvm_conf_tail_backward`, the 3xTF32 GEMMs, the
+BatchNorm backward with one group per pair, `mvm_conf_gather_backward`) into the couplings, before the Sinkhorn
+backward, and into the matching descriptors, before the final projection's backward: stage 2 of training (the pose
+loss).  The forward's outputs and running statistics are bitwise those of `conf_grad=False`, and when no loss reaches
+`conf_scores` the head's backward does not run.  Without `conf_grad` the `conf_scores_*` of `full_output` carry no
+graph.  `matching_scores*` never do (the reference computes them under torch.no_grad())."""
 import torch
 
 from .. import _lib
@@ -159,6 +166,15 @@ def _forward(model, data, view_ids=None, save=False, debug=None):
         raw_all = ops.pair_scores(md, [(slot[id0], slot[id1]) for id0, id1 in pair_list], N)          # [P * B, N+1, N+1]
         Z_all, pot_all = ops.sinkhorn_train_forward(raw_all, alpha, iters, augmented=True)
     pairs_saved = []
+    # conf_grad (train mode, autograd on): keep the confidence head's state of every pair for its backward
+    conf_grad = save and full and bool(cfg['conf_mlp']) and bool(cfg.get('conf_grad', False))
+    conf_saved = {}
+
+    def keep(name, t, p_):
+        # the head's state goes straight into pair-major buffers (rows (p B + b) N + i; statistics one row per pair)
+        if name not in conf_saved:
+            conf_saved[name] = torch.empty((len(pair_list) * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+        conf_saved[name][p_ * t.shape[0]:(p_ + 1) * t.shape[0]].copy_(t)
     for p_, (id0, id1) in enumerate(pair_list):
             a, b_ = slot[id0], slot[id1]
             m0 = md[:, a, :N].contiguous()
@@ -178,14 +194,29 @@ def _forward(model, data, view_ids=None, save=False, debug=None):
                 m1g = m1[bi, i0]                                               # [B, N, 256]
                 add = Z[bi, torch.arange(N, device=dev).unsqueeze(0).expand(B, N), i0].reshape(B * N, 1)
                 cm = model.conf_mlp
-                f = _lin(m0.reshape(B * N, 256), *_conv(cm.layers_f, 0), a2=m1g.reshape(B * N, 256).contiguous())
-                _bn(f, cm.layers_f[1], N, N)
-                f = _bn(_lin(f, *_conv(cm.layers_f, 3)), cm.layers_f[4], N, N)
-                c = _bn(_lin(add.contiguous(), *_conv(cm.layers_c, 0)), cm.layers_c[1], N, N)
-                c = _bn(_lin(c, *_conv(cm.layers_c, 3)), cm.layers_c[4], N, N)
+
+                def head_bn(x, mod):
+                    # conf_grad: out of place with the statistics kept (same kernel, same values); else in place
+                    return _bn(x, mod, N, N, save=True) if conf_grad else (_bn(x, mod, N, N), None)
+                x0, x1 = m0.reshape(B * N, 256), m1g.reshape(B * N, 256).contiguous()
+                pre_f0 = _lin(x0, *_conv(cm.layers_f, 0), a2=x1)
+                y_f1, st_f1 = head_bn(pre_f0, cm.layers_f[1])
+                pre_f3 = _lin(y_f1, *_conv(cm.layers_f, 3))
+                f, st_f4 = head_bn(pre_f3, cm.layers_f[4])
+                add = add.contiguous()
+                pre_c0 = _lin(add, *_conv(cm.layers_c, 0))
+                y_c1, st_c1 = head_bn(pre_c0, cm.layers_c[1])
+                pre_c3 = _lin(y_c1, *_conv(cm.layers_c, 3))
+                c, st_c4 = head_bn(pre_c3, cm.layers_c[4])
                 w_last, b_last = _conv(cm.layers, 0)
-                logit = _lin((f + c).contiguous(), torch.nn.functional.pad(w_last, (0, 0, 0, 15)), torch.nn.functional.pad(b_last, (0, 15)))
+                h_sum = (f + c).contiguous()
+                logit = _lin(h_sum, torch.nn.functional.pad(w_last, (0, 0, 0, 15)), torch.nn.functional.pad(b_last, (0, 15)))
                 conf = torch.sigmoid(logit[:, :1]).reshape(B, N, 1)
+                if conf_grad:
+                    for name, t in dict(m0=x0, m1g=x1, add=add, pre_f0=pre_f0, y_f1=y_f1, st_f1=st_f1, pre_f3=pre_f3,
+                                        y_f4=f, st_f4=st_f4, pre_c0=pre_c0, y_c1=y_c1, st_c1=st_c1, pre_c3=pre_c3, y_c4=c,
+                                        st_c4=st_c4, h=h_sum, conf=conf.reshape(B * N), i0=i0.reshape(B * N)).items():
+                        keep(name, t, p_)
             result['matches{}_{}'.format(id0, key)] = i0
             result['matches{}_{}'.format(id1, key)] = i1
             result['matching_scores{}_{}'.format(id0, key)] = s0
@@ -196,6 +227,7 @@ def _forward(model, data, view_ids=None, save=False, debug=None):
         S.inp, S.kenc, S.kenc_last_in, S.layers, S.x_final, S.md = inp, kenc_saved, h, layers_saved, x, md
         S.pairs, S.alpha, S.iters, S.perm, S.dev = pairs_saved, alpha, iters, perm, dev
         S.raw_all, S.pot_all = raw_all, pot_all
+        S.conf = conf_saved if conf_grad else None
     return result, S
 
 
@@ -209,6 +241,9 @@ def _backward(model, S, grads):
         g = g.reshape(p.shape).to(p.dtype)
         G[p] = g if p not in G else G[p] + g
 
+    # the confidence head's backward runs when it kept its state (conf_grad) and some conf_scores got a gradient
+    conf_g = [grads.get('conf_scores_' + key) for key, _, _ in S.pairs] if S.conf is not None else []
+    head = any(g is not None for g in conf_g)
     with _lib.device_ctx(dev):
         # ---- optimal transport and the score products (multi_view_matcher.py:275-285)
         g_md = torch.zeros(B, T, n_pad, 256, dtype=torch.float32, device=dev)
@@ -217,9 +252,11 @@ def _backward(model, S, grads):
             go = grads.get('scores_' + key)
             if go is not None:
                 G_all[p_ * B:(p_ + 1) * B] = go
+        if head:        # its gradients w.r.t. the couplings and the matching descriptors go in first
+            _conf_backward(model, S, conf_g, g_md, G_all, acc)
         dZ_all, d_alpha = ops.sinkhorn_train_backward(S.raw_all, S.alpha, S.pot_all, S.iters, G_all, augmented=True)      # ONE launch
         for p_, (key, a, b_) in enumerate(S.pairs):
-            if grads.get('scores_' + key) is None:
+            if grads.get('scores_' + key) is None and not (head and conf_g[p_] is not None):
                 continue
             dS = torch.zeros(B, n_pad, n_pad, dtype=torch.float32, device=dev)
             dS[:, :N, :N] = dZ_all[p_ * B:(p_ + 1) * B, :N, :N]
@@ -296,6 +333,59 @@ def _backward(model, S, grads):
     return G
 
 
+def _conf_backward(model, S, conf_g, g_md, G_all, acc):
+    """Backward of ConfidenceMLP (multi_view_matcher.py:39-53, 302-306) over every pair at once, on the pair-major
+    buffers the forward filled (rows r = (p B + b) N + i).  conf_g: per pair the gradient w.r.t. conf_scores
+    [B, N, 1] or None (zero).  Adds the gradients w.r.t. the gathered inputs to g_md [B, T, n_pad, 256] (m0, m1g) and
+    G_all [P B, N+1, N+1] (add), and the parameter gradients through acc.  Each pair's BatchNorms took their statistics over its own B N rows: one group
+    per pair (slot size B N)."""
+    B, T, N, n_pad, rows, g_bn = S.dims
+    cm = model.conf_mlp
+    P = len(S.pairs)
+    sv = S.conf
+    dbg = getattr(model, '_train_debug', None)      # tests: the head's gradients at its stage boundaries
+    g_conf = torch.cat([(g.detach().float() if g is not None else torch.zeros(B, N, 1, device=S.dev)).reshape(-1)
+                        for g in conf_g])
+    # sigmoid' and the 256 -> 1 layer (csrc/conf_train.cu)
+    g_h, dw_last, db_last = ops.conf_tail_backward(sv['conf'], g_conf, sv['h'], cm.layers[0].weight[:, :, 0])
+    acc(cm.layers[0].weight, dw_last)
+    acc(cm.layers[0].bias, db_last)
+    bn_rows = B * N
+    g_x = g_pre_c0 = None
+    for br, mods in (('f', cm.layers_f), ('c', cm.layers_c)):
+        g = g_h.clone() if br == 'f' else g_h         # the BatchNorm backward runs in place
+        if dbg is not None:
+            dbg.setdefault('conf', {})['g_h'] = g_h.clone()
+        dg, db = ops.batchnorm_train_backward(sv['pre_%s3' % br], sv['y_%s4' % br], g,
+                                              mods[4].weight.detach().float().contiguous(), sv['st_%s4' % br],
+                                              bn_rows, bn_rows)
+        acc(mods[4].weight, dg)
+        acc(mods[4].bias, db)
+        acc(mods[3].weight, ops.gemm_dw(g, sv['y_%s1' % br]))
+        acc(mods[3].bias, ops.colsum(g))
+        g1 = ops.gemm_dx(g, mods[3].weight[:, :, 0])
+        if dbg is not None:
+            dbg['conf'].update({'g_pre_%s3' % br: g.clone(), 'g_y_%s1' % br: g1.clone()})
+        dg, db = ops.batchnorm_train_backward(sv['pre_%s0' % br], sv['y_%s1' % br], g1,
+                                              mods[1].weight.detach().float().contiguous(), sv['st_%s1' % br],
+                                              bn_rows, bn_rows)
+        acc(mods[1].weight, dg)
+        acc(mods[1].bias, db)
+        if dbg is not None:
+            dbg['conf'].update({'g_pre_%s0' % br: g1.clone(), 'dgamma_%s1' % br: dg.clone()})
+        acc(mods[0].bias, ops.colsum(g1))
+        if br == 'f':
+            acc(mods[0].weight, ops.gemm_dw(g1, sv['m0'], sv['m1g']))
+            g_x = ops.gemm_dx(g1, mods[0].weight[:, :, 0])                  # [rows, 512]: m0 | m1g
+        else:
+            g_pre_c0 = g1
+    # the gathers' transposes and the score-input layer (K = 1) (csrc/conf_train.cu)
+    i0 = sv['i0'].view(P, B, N)
+    dw_c0 = ops.conf_gather_backward(g_x, g_pre_c0, sv['add'], cm.layers_c[0].weight[:, 0, 0], i0,
+                                     [(a, b_) for _, a, b_ in S.pairs], g_md, G_all)
+    acc(cm.layers_c[0].weight, dw_c0)
+
+
 class MatcherTrainFn(torch.autograd.Function):
     """(model, data, view_ids, holder, *parameters) -> the coupling matrices of every pair; the non-differentiable
     outputs of `full_output` are left in `holder`."""
@@ -304,7 +394,12 @@ class MatcherTrainFn(torch.autograd.Function):
     def forward(ctx, model, data, view_ids, holder, *params):
         result, S = _forward(model, data, view_ids, save=True)
         keys = [k for k in result if k.startswith('scores_')]
-        holder.update({k: v for k, v in result.items() if not k.startswith('scores_')})
+        if S.conf is not None:          # conf_grad: the confidences are differentiable outputs too
+            keys += [k for k in result if k.startswith('conf_scores_')]
+            # an output without a gradient arrives as None, not zeros: the confidence head's backward runs only when a
+            # loss reaches conf_scores
+            ctx.set_materialize_grads(False)
+        holder.update({k: v for k, v in result.items() if k not in keys})
         holder['__keys__'] = keys
         ctx.model, ctx.S, ctx.keys, ctx.params = model, S, keys, params
         return tuple(result[k] for k in keys)

@@ -396,3 +396,51 @@ def sinkhorn_train_backward(scores, alpha, pot, iters, grad_out, augmented=False
                                                int(iters), _lib.ptr(dZ), _lib.ptr(d_alpha), _lib.stream_ptr()),
                'mvm_sinkhorn_train_backward')
     return dZ, d_alpha
+
+
+# ---- backward of the ConfidenceMLP (stage 2 of training): csrc/conf_train.cu ---------------------------------------------
+
+def conf_tail_backward(conf, g_conf, h, w_last):
+    """sigmoid' and the 256 -> 1 layer of the confidence head: conf / g_conf [rows] (sigmoid outputs and their gradient),
+    h [rows, 256] (its input), w_last [256] -> (g_h [rows, 256], dW_last [256], db_last [1]) (mvm_conf_tail_backward)."""
+    lib = _lib.lib()
+    rows = h.shape[0]
+    assert h.shape == (rows, 256) and conf.numel() == rows and g_conf.numel() == rows and w_last.numel() == 256
+    dev = h.device
+    g_h = torch.empty(rows, 256, dtype=torch.float32, device=dev)
+    dw = torch.empty(256, dtype=torch.float32, device=dev)
+    db = torch.empty(1, dtype=torch.float32, device=dev)
+    nws = lib.mvm_conf_backward_ws_doubles(rows)
+    ws = torch.empty(nws, dtype=torch.float64, device=dev)
+    f = lambda t: t.detach().float().reshape(-1).contiguous()
+    _lib.check(lib.mvm_conf_tail_backward(_lib.ptr(f(conf)), _lib.ptr(f(g_conf)), _lib.ptr(h.contiguous()),
+                                          _lib.ptr(f(w_last)), rows, _lib.ptr(g_h), _lib.ptr(dw), _lib.ptr(db),
+                                          _lib.ptr(ws), nws, _lib.stream_ptr()), 'mvm_conf_tail_backward')
+    return g_h, dw, db
+
+
+def conf_gather_backward(g_x, g_pre_c0, add, w_c0, i0, pairs, g_md, g_scores):
+    """Transposes of the confidence head's input gathers (mvm_conf_gather_backward), pair-major rows r = (p B + b) N + i:
+    g_x [rows, 512] (gradient w.r.t. cat[m0, m1g]), g_pre_c0 [rows, 256] (w.r.t. the score-input layer's output),
+    add [rows] and w_c0 [256] (that layer's input and weight), i0 [P, B, N] int64, pairs [(slot a, slot b)].  In place:
+    g_md [B, T, n_pad, 256] += the m0 / m1g terms, g_scores [P * B, N + 1, N + 1] += the score-input term at
+    [i, i0 (-1 -> N)].  -> dW_c0 [256]."""
+    lib = _lib.lib()
+    P, B, N = i0.shape
+    _, T, n_pad, _ = g_md.shape
+    rows = P * B * N
+    assert len(pairs) == P and g_x.shape == (rows, 512) and g_pre_c0.shape == (rows, 256) and add.numel() == rows
+    assert g_md.is_contiguous() and g_scores.is_contiguous() and g_scores.shape == (P * B, N + 1, N + 1)
+    dev = g_x.device
+    dw = torch.empty(256, dtype=torch.float32, device=dev)
+    nws = lib.mvm_conf_backward_ws_doubles(rows)
+    ws = torch.empty(nws, dtype=torch.float64, device=dev)
+    I = C.c_int * P
+    _lib.check(lib.mvm_conf_gather_backward(_lib.ptr(g_x.contiguous()), _lib.ptr(g_pre_c0.contiguous()),
+                                            _lib.ptr(add.detach().float().reshape(-1).contiguous()),
+                                            _lib.ptr(w_c0.detach().float().reshape(-1).contiguous()),
+                                            _lib.ptr(i0.long().contiguous()), P, B, N, T, n_pad,
+                                            I(*[a for a, _ in pairs]), I(*[b for _, b in pairs]), _lib.ptr(g_md),
+                                            _lib.ptr(g_scores), _lib.ptr(dw), _lib.ptr(ws), nws, _lib.stream_ptr()),
+               'mvm_conf_gather_backward')
+    return dw

@@ -21,10 +21,14 @@ Built:
   * LogOptimalTransport: autograd.Function over mvm_sinkhorn_train_{forward,backward} -- the exact gradient of the 100
     unrolled iterations (what autograd computes for the reference, superglue.py:143-172), with respect to the scores
     and to bin_score.
-The weighted eight-point is differentiable with respect to the match confidences
-(pose_optimization/two_view/estimate_relative_pose.py, mvm_w8pt_backward), so the pose losses of run_matcher carry a
-graph as far as conf_scores.  Not built (stated, not hidden): the rest of stage 2 of cfg5 (--pose_loss): the backward of
-the ConfidenceMLP, the graph through the train-mode full_output, and train_step with opt.pose_loss (it raises).
+  * the TRAINING step of stage 2 (train.py:405-426 with --pose_loss): run_matcher with `conf_grad`, so the rotation /
+    translation losses of the weighted eight-point (pose_optimization/two_view/estimate_relative_pose.py,
+    mvm_w8pt_backward) reach conf_scores and, through the ConfidenceMLP's backward (models/train_forward.py,
+    csrc/conf_train.cu), the confidence head and the matcher; the step is skipped unless every gradient is finite
+    after the all-reduce (has_finite_gradients); get_parameters builds the reference's two optimiser groups and
+    next_pose_match_ratio is its pose_match_ratio ramp.
+Not built: gradients through the two-view BA or with respect to keypoints, intrinsics or the target (the reference's
+stage 2 does not take them either), and loading a stage-1 optimiser state into the two-group optimiser (load_ckpt).
 """
 import torch
 
@@ -199,13 +203,15 @@ def compute_gt_matches(opt, data):
 
 def run_matcher(opt, data, matcher):
     """helpers.py:243-260.  Eval mode = the validation pass (train.py:66-68); train mode = the training step, where the
-    match loss carries MatcherTrainFn's graph.  The pose losses carry a graph through the weighted eight-point as far
-    as conf_scores when those require grad; the train-mode conf_scores have none yet (the confidence head's backward
-    is not built), so in train mode the pose losses still reach no parameter."""
+    match loss carries MatcherTrainFn's graph.  With opt.pose_loss the matcher runs with `full_output` and `conf_grad`
+    (the reference sets full_output the same way, helpers.py:245): in train mode under autograd the conf_scores carry
+    MatcherTrainFn's graph, so the rotation / translation losses reach the confidence head and, through its inputs,
+    the matcher -- the weighted eight-point's backward (mvm_w8pt_backward), then the head's (csrc/conf_train.cu)."""
     from .pose_optimization.two_view.estimate_relative_pose import run_weighted_8_point
     from .pose_optimization.two_view.compute_pose_error import compute_rotation_error, compute_translation_error_as_angle
     curr_tuple_size = len(data["ids"])
-    getattr(matcher, 'module', matcher).config["full_output"] = opt.pose_loss        # DataParallel / DDP wrapped or bare
+    m = getattr(matcher, 'module', matcher)                                            # DataParallel / DDP wrapped or bare
+    m.config["full_output"] = opt.pose_loss; m.config["conf_grad"] = opt.pose_loss
     result = matcher(data)
     match_loss = torch.zeros(1, device=data["pose0"].device)
     rot_loss = torch.zeros(1, device=match_loss.device)
@@ -243,15 +249,61 @@ def validation_step(opt, data, matcher, n_pairs, pose_match_ratio, process_group
     return val_loss, losses
 
 
+def get_parameters(model, whitelist_key=None, blacklist_key=None):
+    """helpers.py:63-71: the parameters whose name contains `whitelist_key` (when given) and not `blacklist_key`
+    (when given), in named_parameters() order.  The reference's stage-2 optimiser (train.py:360-362) is
+    Adam(get_parameters(m, blacklist_key="conf_mlp"), lr) plus the group get_parameters(m, whitelist_key="conf_mlp")
+    at lr 1e-4."""
+    params = []
+    for n, param in model.named_parameters():
+        if whitelist_key is not None and whitelist_key not in n:
+            continue
+        if blacklist_key is not None and blacklist_key in n:
+            continue
+        params.append(param)
+    return params
+
+
+def _all_finite(params):
+    """One device-side test over every existing gradient of `params` -> 0-dim bool tensor (no host synchronisation)."""
+    grads = [p.grad.reshape(-1) for p in params if p.grad is not None]
+    if not grads:
+        return torch.ones((), dtype=torch.bool)
+    return torch.isfinite(torch.cat(grads)).all()
+
+
+def has_finite_gradients(model):
+    """helpers.py:284-288: False when some parameter's gradient holds an inf or a NaN.  One host synchronisation."""
+    return bool(_all_finite(list(model.parameters())))
+
+
+POSE_MATCH_RATIO_INCREMENT = 2.5e-5
+
+
+def next_pose_match_ratio(pose_match_ratio, final_pose_match_ratio, increment=POSE_MATCH_RATIO_INCREMENT):
+    """The stage-2 ramp of train.py:414-416, applied once per training step before combine_losses: while the ratio
+    is below `final_pose_match_ratio` it grows by `increment`, capped at 1."""
+    if pose_match_ratio < final_pose_match_ratio:
+        pose_match_ratio = min(pose_match_ratio + increment, 1.)
+    return pose_match_ratio
+
+
 def train_step(opt, data, matcher, optimizer, n_pairs, pose_match_ratio=0.0, grad_clip=-1.0, super_point=None):
-    """One iteration of the training loop (train.py:409-426), stage 1 (match loss): run_super_point when the batch
-    carries images and no keypoints (then `super_point` is required), ground-truth matches when it still carries depth
-    maps, run_matcher in train mode, combine_losses, backward through the kernels, gradient averaging over the ranks
-    when torch.distributed is initialised (DistributedDataParallel's all-reduce in the reference), optional value
-    clipping, optimiser step.  -> (train_loss tensor, losses dict)."""
-    if getattr(opt, 'pose_loss', False):
-        raise NotImplementedError('stage 2 (--pose_loss) needs the gradients of the pose stage, which are not built')
+    """One iteration of the training loop (train.py:409-426): run_super_point when the batch carries images and no
+    keypoints (then `super_point` is required), ground-truth matches when it still carries depth maps, run_matcher in
+    train mode, combine_losses, backward through the kernels, gradient averaging over the ranks when
+    torch.distributed is initialised (DistributedDataParallel's all-reduce in the reference), optional value clipping,
+    optimiser step.
+
+    Stage 1 (opt.pose_loss False): the match loss alone.  Stage 2 (opt.pose_loss): run_matcher adds the rotation and
+    translation losses of the weighted eight-point with choose_closest against the ground-truth pose, and their
+    gradient reaches the confidence head and the matcher; `pose_match_ratio` (see next_pose_match_ratio) weighs them
+    against the match loss with opt.rot_weight / opt.trans_weight.  The step is applied only when every gradient of the
+    optimiser's parameters is finite after the all-reduce (the reference's has_finite_gradients), so every rank takes
+    the same decision; the test costs one host synchronisation.  -> (train_loss tensor, losses dict); with pose_loss the
+    dict also holds `finite_gradients`, a bool tensor (False: the step was skipped)."""
     from . import sharding
+    pose = bool(getattr(opt, 'pose_loss', False))
     if _images_in(data, super_point):
         run_super_point(opt, data, super_point)
     if "depth0" in data:
@@ -264,7 +316,12 @@ def train_step(opt, data, matcher, optimizer, n_pairs, pose_match_ratio=0.0, gra
     train_loss.backward()
     params = [p for group in optimizer.param_groups for p in group['params']]
     sharding.all_reduce_gradients(params)
-    if grad_clip > 0.0:
-        torch.nn.utils.clip_grad_value_(params, grad_clip)
-    optimizer.step()
-    return train_loss.detach(), {k: v.detach() for k, v in losses.items()}
+    finite = _all_finite(params) if pose else None
+    if finite is None or bool(finite):
+        if grad_clip > 0.0:
+            torch.nn.utils.clip_grad_value_(params, grad_clip)
+        optimizer.step()
+    out = {k: v.detach() for k, v in losses.items()}
+    if pose:
+        out["finite_gradients"] = finite.reshape(())
+    return train_loss.detach(), out

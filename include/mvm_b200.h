@@ -496,6 +496,30 @@ int mvm_batchnorm_train_backward(const float* x, const float* y, float* dy, int 
                                  float* dgamma, float* dbeta, int accumulate, double* ws, void* stream);
 /* out[c] (+)= sum_r x[r, c]: the bias gradient of a Conv1d(k=1) from the gradient of its output.  ws: C doubles. */
 int mvm_colsum(const float* x, int rows, int C, int ld, float* out, int accumulate, double* ws, void* stream);
+/* Backward of the ConfidenceMLP of the train branch (stage 2 of training; multi_view_matcher.py:39-53, 302-306), the two
+ * steps the GEMM / BatchNorm / colsum kernels do not cover.  Rows are pair-major, r = (p * batch + b) * n + i.  Both are
+ * deterministic (fixed summation order, fp64 accumulators, no floating-point atomics).  ws: mvm_conf_backward_ws_doubles(rows).
+ * Tail: conf [rows] = the sigmoid outputs, g_conf [rows] = the gradient w.r.t. them, h [rows, 256] = out_f + out_c,
+ * w_last [256] -> g_h [rows, 256] = g_conf c (1 - c) w_last, dw_last [256] and db_last [1] (overwritten). */
+#define MVM_CONF_MAX_PAIRS 28
+size_t mvm_conf_backward_ws_doubles(int rows);
+int mvm_conf_tail_backward(const float* conf, const float* g_conf, const float* h, const float* w_last, int rows,
+                           float* g_h, float* dw_last, float* db_last, double* ws, size_t ws_doubles, void* stream);
+/* Gather transpose: g_x [rows, 512] = the gradient w.r.t. cat[m0, m1g]; g_pre_c0 [rows, 256] = the gradient w.r.t. the
+ * pre-BatchNorm output of the score-input layer (K = 1), add [rows] its input, w_c0 [256] its weight; i0 [rows] int64 in
+ * [-1, n).  slot_a / slot_b: host arrays (n_pairs <= MVM_CONF_MAX_PAIRS) of the pairs' view slots.  Adds
+ * g_x[r, :256] to g_md[b, slot_a[p], i] and g_x[r, 256:] to g_md[b, slot_b[p], i0 (-1 -> n - 1)] (g_md [batch, n_views,
+ * n_pad, 256]; rows without a contribution are not written), sum_k g_pre_c0[r, k] w_c0[k] to
+ * g_scores[p * batch + b, i, i0 (-1 -> n)] (g_scores [n_pairs * batch, n + 1, n + 1]), and writes dw_c0[k] =
+ * sum_r g_pre_c0[r, k] add[r].  The range of i0 is read back (one stream synchronisation) and checked before the
+ * gathers launch. */
+int mvm_conf_gather_backward(const float* g_x, const float* g_pre_c0, const float* add, const float* w_c0,
+                             const int64_t* i0, int n_pairs, int batch, int n, int n_views, int n_pad, const int* slot_a,
+                             const int* slot_b, float* g_md, float* g_scores, float* dw_c0, double* ws, size_t ws_doubles,
+                             void* stream);
+/* A / B hook (process-wide): 0 skips the read-back of the i0 range in mvm_conf_gather_backward (the caller then
+ * guarantees i0 in [-1, n)); default 1. */
+void mvm_debug_set_conf_i0_check(int on);
 /* x [R, C] (row stride ld) -> transposed copies [C, R] (row stride ldo): raw (may be NULL) and / or the tf32 planes
  * hi = rn_tf32(x), lo = rn_tf32(x - hi) (both or neither) that mvm_linear_tc_presplit takes as its W operand: the operand
  * staging of the backward GEMMs (dX = dY W: W^T planes; dW = dY^T X: dY^T raw and X^T planes). */
