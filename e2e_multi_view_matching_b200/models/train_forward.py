@@ -13,15 +13,16 @@ The whole matcher is ONE autograd.Function (`MatcherTrainFn`): its inputs are th
 coupling matrices, so `loss.backward()`, torch optimisers and DistributedDataParallel's gradient hooks work unchanged.
 
 The confidence head's graph is opt-in, through the matcher config key `conf_grad` (default False; training.run_matcher
-sets it to opt.pose_loss, like `full_output`).  With `full_output` and `conf_grad` in train mode under autograd, the
-forward keeps the head's state of every pair (its inputs m0, m1g and the score input, the pre- and post-BatchNorm
-activations and statistics, h = out_f + out_c, the sigmoid output, the matches) and `conf_scores_*` are differentiable
-outputs beside `scores_*`.  Their gradient runs back through the head (`mvm_conf_tail_backward`, the 3xTF32 GEMMs, the
-BatchNorm backward with one group per pair, `mvm_conf_gather_backward`) into the couplings, before the Sinkhorn
-backward, and into the matching descriptors, before the final projection's backward: stage 2 of training (the pose
-loss).  The forward's outputs and running statistics are bitwise those of `conf_grad=False`, and when no loss reaches
-`conf_scores` the head's backward does not run.  Without `conf_grad` the `conf_scores_*` of `full_output` carry no
-graph.  `matching_scores*` never do (the reference computes them under torch.no_grad())."""
+sets it to opt.pose_loss, like `full_output`).  The head runs once over the rows of every pair (pair-major, one
+BatchNorm group per pair).  With `full_output` and `conf_grad` in train mode under autograd, the forward keeps its state
+(the records of its four Conv1d + BatchNorm + ReLU blocks, which hold the inputs m0 | m1g and the score input, the pre-
+and post-BatchNorm activations and statistics; h = out_f + out_c, the sigmoid output, the matches) and `conf_scores_*`
+are differentiable outputs beside `scores_*`.  Their gradient runs back through the head (`mvm_conf_tail_backward`,
+the 3xTF32 GEMMs, the BatchNorm backward with one group per pair, `mvm_conf_gather_backward`) into the couplings,
+before the Sinkhorn backward, and into the matching descriptors, before the final projection's backward: stage 2 of
+training (the pose loss).  The forward's outputs and running statistics are bitwise those of `conf_grad=False`, and
+when no loss reaches `conf_scores` the head's backward does not run.  Without `conf_grad` the `conf_scores_*` of
+`full_output` carry no graph.  `matching_scores*` never do (the reference computes them under torch.no_grad())."""
 import torch
 
 from .. import _lib
@@ -54,19 +55,43 @@ def _lin(x, w, b, relu=False, a2=None, residual=None, alpha=1.0):
     return ops.linear(x, w, bias=b, a2=a2, residual=residual, relu=relu, alpha=alpha, tc_passes=0)
 
 
-def _bn(x, bn, n_pad, n_valid, relu=True, groups=1, save=False):
-    """nn.BatchNorm1d in training mode on x [rows, C]; updates the module's running statistics.  groups > 1: the view
-    slots s = g (mod groups) are normalised one group after the other (one BatchNorm call per view, as the pairwise
-    train path makes them).  save: out of place (padding rows of y = 0: the weight-gradient GEMMs contract over them), ->
-    (y, saved statistics) for the backward; else in place -> y."""
+def _block(x, w, b, bn, n_pad, n_valid, groups=1, a2=None, save=False):
+    """Conv1d(k=1) of [x | a2] -> nn.BatchNorm1d in training mode -> ReLU on point-major rows; updates the BatchNorm's
+    running statistics.  groups > 1: the slots s = g (mod groups) of n_pad rows are normalised one group after the other
+    (one BatchNorm call per view, as the pairwise train path makes them; one per pair in the confidence head).  save:
+    the BatchNorm runs out of place (padding rows of y = 0: the weight-gradient GEMMs contract over them), else in
+    place.
+    -> (y, record (x, a2, pre-BatchNorm activation, y, statistics) for _block_backward, or None without save)."""
     assert bn.weight is not None and bn.track_running_stats
+    pre = _lin(x, w, b, a2=a2)
     momentum = 0.1 if bn.momentum is None else bn.momentum
-    with _lib.device_ctx(x.device):
-        y, stats = ops.batchnorm_train(x, bn.weight.detach().float().contiguous(), bn.bias.detach().float().contiguous(),
-                                       bn.running_mean, bn.running_var, momentum, bn.eps, n_pad, n_valid, relu=relu,
-                                       groups=groups, out=torch.zeros_like(x) if save else None, save=save)
+    with _lib.device_ctx(pre.device):
+        y, stats = ops.batchnorm_train(pre, bn.weight.detach().float().contiguous(),
+                                       bn.bias.detach().float().contiguous(), bn.running_mean, bn.running_var,
+                                       momentum, bn.eps, n_pad, n_valid, relu=True, groups=groups,
+                                       out=torch.zeros_like(pre) if save else None, save=save)
     bn.num_batches_tracked += groups
-    return (y, stats) if save else y
+    return y, ((x, a2, pre, y, stats) if save else None)
+
+
+def _bn_backward(rec, bn, g, n_pad, n_valid, acc):
+    """Backward of the BatchNorm and ReLU of a _block record, in place on g (gradient w.r.t. the block's output ->
+    w.r.t. its pre-BatchNorm activation); the BatchNorm's parameter gradients go through acc.  -> dgamma."""
+    _, _, pre, y, stats = rec
+    dg, db = ops.batchnorm_train_backward(pre, y, g, bn.weight.detach().float().contiguous(), stats, n_pad, n_valid)
+    acc(bn.weight, dg)
+    acc(bn.bias, db)
+    return dg
+
+
+def _block_backward(rec, conv, bn, g, n_pad, n_valid, acc):
+    """Backward of _block from the gradient g w.r.t. its output (overwritten, see _bn_backward): the parameter gradients
+    go through acc -> the gradient w.r.t. its input [x | a2]."""
+    x, a2 = rec[:2]
+    _bn_backward(rec, bn, g, n_pad, n_valid, acc)
+    acc(conv.weight, ops.gemm_dw(g, x, a2))
+    acc(conv.bias, ops.colsum(g))
+    return ops.gemm_dx(g, conv.weight[:, :, 0])
 
 
 def _conv(seq, i):
@@ -115,13 +140,8 @@ def _forward(model, data, view_ids=None, save=False, debug=None):
         w, b = _conv(enc, i)
         if i == 0:
             w = torch.nn.functional.pad(w, (0, 13))
-        pre = _lin(h, w, b)
-        if save:
-            y, st = _bn(pre, enc[i + 1], n_pad, N, groups=g_bn, save=True)
-            kenc_saved.append((h, pre, y, st))
-            h = y
-        else:
-            h = _bn(pre, enc[i + 1], n_pad, N, groups=g_bn)
+        h, rec = _block(h, w, b, enc[i + 1], n_pad, N, groups=g_bn, save=save)
+        kenc_saved.append(rec)
     x = _lin(h, *_conv(enc, 12), residual=x_desc)                            # desc + kenc(kpts, scores)
     if debug is not None:
         debug['kenc'] = (x - x_desc).view(B, T, n_pad, 256)[:, :, :N].clone()
@@ -136,12 +156,9 @@ def _forward(model, data, view_ids=None, save=False, debug=None):
         qkv = _lin(x, wqkv, bqkv)
         msg = ops.attention(qkv.view(B * T, n_pad, 768), B, T, counts, 1 if name == 'cross' else 0, tc_passes='h3')
         merged = _lin(msg.view(rows, 256), attn.merge.weight[:, :, 0][:, perm], attn.merge.bias)
-        hid_pre = _lin(x, *_conv(layer.mlp, 0), a2=merged)
+        hid, rec = _block(x, *_conv(layer.mlp, 0), layer.mlp[1], n_pad, N, groups=g_bn, a2=merged, save=save)
         if save:
-            hid, st = _bn(hid_pre, layer.mlp[1], n_pad, N, groups=g_bn, save=True)
-            layers_saved.append((x, qkv, msg, merged, hid_pre, hid, st, name))
-        else:
-            hid = _bn(hid_pre, layer.mlp[1], n_pad, N, groups=g_bn)
+            layers_saved.append((qkv, msg, rec, name))
         x_new = _lin(hid, *_conv(layer.mlp, 3), residual=x)                  # desc + delta (multi_view_matcher.py:80,83)
         if debug is not None and 'layer0_delta' not in debug:
             debug['layer0_delta'] = (x_new - x).view(B, T, n_pad, 256)[:, :, :N].clone()
@@ -162,73 +179,63 @@ def _forward(model, data, view_ids=None, save=False, debug=None):
     # training kernel keeps the potentials of every iteration; couplings of an untrained / early-training network span
     # thousands of nats, beyond the range of the scaling-domain kernels of the eval path.
     pair_list = [(id0, id1) for id1 in ids for id0 in ids if id0 < id1]
+    pair_slots = [(slot[id0], slot[id1]) for id0, id1 in pair_list]
     with _lib.device_ctx(dev):
-        raw_all = ops.pair_scores(md, [(slot[id0], slot[id1]) for id0, id1 in pair_list], N)          # [P * B, N+1, N+1]
+        raw_all = ops.pair_scores(md, pair_slots, N)                                       # [P * B, N+1, N+1]
         Z_all, pot_all = ops.sinkhorn_train_forward(raw_all, alpha, iters, augmented=True)
-    pairs_saved = []
-    # conf_grad (train mode, autograd on): keep the confidence head's state of every pair for its backward
+    # conf_grad (train mode, autograd on): keep the confidence head's state for its backward
     conf_grad = save and full and bool(cfg['conf_mlp']) and bool(cfg.get('conf_grad', False))
-    conf_saved = {}
-
-    def keep(name, t, p_):
-        # the head's state goes straight into pair-major buffers (rows (p B + b) N + i; statistics one row per pair)
-        if name not in conf_saved:
-            conf_saved[name] = torch.empty((len(pair_list) * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
-        conf_saved[name][p_ * t.shape[0]:(p_ + 1) * t.shape[0]].copy_(t)
+    conf = conf_saved = None
+    if full:
+        i0, i1, s0, s1 = ops.extract_matches(Z_all, model.match_threshold)               # every pair: [P * B, N]
+        if cfg['conf_mlp']:
+            conf, conf_saved = _conf_forward(model, md, Z_all, i0, pair_slots, conf_grad)
     for p_, (id0, id1) in enumerate(pair_list):
-            a, b_ = slot[id0], slot[id1]
-            m0 = md[:, a, :N].contiguous()
-            m1 = md[:, b_, :N].contiguous()
-            Z = Z_all[p_ * B:(p_ + 1) * B]
-            key = '{}_{}'.format(id0, id1)
-            result['scores_' + key] = Z
-            if save:
-                pairs_saved.append((key, a, b_))
-            if not full:
-                continue
-            i0, i1, s0, s1 = ops.extract_matches(Z, model.match_threshold)
-            conf = None
-            if cfg['conf_mlp']:
-                # inputs of ConfidenceMLP (multi_view_matcher.py:302-306): -1 wraps to the last keypoint / dustbin column
-                bi = torch.arange(B, device=dev).unsqueeze(-1).expand(B, N)
-                m1g = m1[bi, i0]                                               # [B, N, 256]
-                add = Z[bi, torch.arange(N, device=dev).unsqueeze(0).expand(B, N), i0].reshape(B * N, 1)
-                cm = model.conf_mlp
-
-                def head_bn(x, mod):
-                    # conf_grad: out of place with the statistics kept (same kernel, same values); else in place
-                    return _bn(x, mod, N, N, save=True) if conf_grad else (_bn(x, mod, N, N), None)
-                x0, x1 = m0.reshape(B * N, 256), m1g.reshape(B * N, 256).contiguous()
-                pre_f0 = _lin(x0, *_conv(cm.layers_f, 0), a2=x1)
-                y_f1, st_f1 = head_bn(pre_f0, cm.layers_f[1])
-                pre_f3 = _lin(y_f1, *_conv(cm.layers_f, 3))
-                f, st_f4 = head_bn(pre_f3, cm.layers_f[4])
-                add = add.contiguous()
-                pre_c0 = _lin(add, *_conv(cm.layers_c, 0))
-                y_c1, st_c1 = head_bn(pre_c0, cm.layers_c[1])
-                pre_c3 = _lin(y_c1, *_conv(cm.layers_c, 3))
-                c, st_c4 = head_bn(pre_c3, cm.layers_c[4])
-                w_last, b_last = _conv(cm.layers, 0)
-                h_sum = (f + c).contiguous()
-                logit = _lin(h_sum, torch.nn.functional.pad(w_last, (0, 0, 0, 15)), torch.nn.functional.pad(b_last, (0, 15)))
-                conf = torch.sigmoid(logit[:, :1]).reshape(B, N, 1)
-                if conf_grad:
-                    for name, t in dict(m0=x0, m1g=x1, add=add, pre_f0=pre_f0, y_f1=y_f1, st_f1=st_f1, pre_f3=pre_f3,
-                                        y_f4=f, st_f4=st_f4, pre_c0=pre_c0, y_c1=y_c1, st_c1=st_c1, pre_c3=pre_c3, y_c4=c,
-                                        st_c4=st_c4, h=h_sum, conf=conf.reshape(B * N), i0=i0.reshape(B * N)).items():
-                        keep(name, t, p_)
-            result['matches{}_{}'.format(id0, key)] = i0
-            result['matches{}_{}'.format(id1, key)] = i1
-            result['matching_scores{}_{}'.format(id0, key)] = s0
-            result['matching_scores{}_{}'.format(id1, key)] = s1
-            result['conf_scores_' + key] = conf
+        key = '{}_{}'.format(id0, id1)
+        pb = slice(p_ * B, (p_ + 1) * B)
+        result['scores_' + key] = Z_all[pb]
+        if full:
+            result['matches{}_{}'.format(id0, key)] = i0[pb]
+            result['matches{}_{}'.format(id1, key)] = i1[pb]
+            result['matching_scores{}_{}'.format(id0, key)] = s0[pb]
+            result['matching_scores{}_{}'.format(id1, key)] = s1[pb]
+            result['conf_scores_' + key] = None if conf is None else conf[pb]
     if save:
         S.dims = (B, T, N, n_pad, rows, g_bn)
-        S.inp, S.kenc, S.kenc_last_in, S.layers, S.x_final, S.md = inp, kenc_saved, h, layers_saved, x, md
-        S.pairs, S.alpha, S.iters, S.perm, S.dev = pairs_saved, alpha, iters, perm, dev
+        S.kenc, S.kenc_last_in, S.layers, S.x_final, S.md = kenc_saved, h, layers_saved, x, md
+        S.pairs = [('{}_{}'.format(id0, id1), a, b_) for (id0, id1), (a, b_) in zip(pair_list, pair_slots)]
+        S.alpha, S.iters, S.perm, S.dev = alpha, iters, perm, dev
         S.raw_all, S.pot_all = raw_all, pot_all
-        S.conf = conf_saved if conf_grad else None
+        S.conf = conf_saved
     return result, S
+
+
+def _conf_forward(model, md, Z_all, i0, pairs, save):
+    """ConfidenceMLP (multi_view_matcher.py:39-53, 302-306) of every pair at once, on pair-major rows
+    r = (p B + b) N + i: md [B, T, n_pad, 256] matching descriptors, Z_all [P B, N+1, N+1] couplings and i0 [P B, N]
+    matches of the pairs [(slot a, slot b)].  Each pair's BatchNorms take their statistics over its own B N rows (one
+    group per pair, whose running statistics are applied pair after pair).  -> (confidences [P B, N, 1], the head's
+    state for _conf_backward or None without save)."""
+    cm = model.conf_mlp
+    B, P, N = md.shape[0], len(pairs), i0.shape[1]
+    dev = md.device
+    n = B * N
+    # inputs (multi_view_matcher.py:302-306): m0, m1g = m1[b, i0], add = scores[b, i, i0]; -1 wraps to the last
+    # keypoint / the dustbin column
+    m0 = torch.stack([md[:, a, :N] for a, _ in pairs]).view(P * n, 256)
+    m1 = torch.stack([md[:, b_, :N] for _, b_ in pairs])                                       # [P, B, N, 256]
+    m1g = m1[torch.arange(P, device=dev).view(P, 1, 1), torch.arange(B, device=dev).view(1, B, 1), i0.view(P, B, N)]
+    add = Z_all[torch.arange(P * B, device=dev).unsqueeze(-1), torch.arange(N, device=dev), i0].view(P * n, 1)
+    y_f1, f1 = _block(m0, *_conv(cm.layers_f, 0), cm.layers_f[1], n, n, groups=P, a2=m1g.view(P * n, 256), save=save)
+    f, f4 = _block(y_f1, *_conv(cm.layers_f, 3), cm.layers_f[4], n, n, groups=P, save=save)
+    y_c1, c1 = _block(add, *_conv(cm.layers_c, 0), cm.layers_c[1], n, n, groups=P, save=save)
+    c, c4 = _block(y_c1, *_conv(cm.layers_c, 3), cm.layers_c[4], n, n, groups=P, save=save)
+    w_last, b_last = _conv(cm.layers, 0)
+    h = f + c
+    logit = _lin(h, torch.nn.functional.pad(w_last, (0, 0, 0, 15)), torch.nn.functional.pad(b_last, (0, 15)))
+    conf = torch.sigmoid(logit[:, :1])
+    saved = dict(f=(f1, f4), c=(c1, c4), h=h, conf=conf.view(P * n), i0=i0.view(P * n)) if save else None
+    return conf.view(P * B, N, 1), saved
 
 
 def _backward(model, S, grads):
@@ -282,16 +289,14 @@ def _backward(model, S, grads):
         # ---- GNN layers, last to first (superglue.py:94-121, multi_view_matcher.py:65-86)
         inv = torch.empty_like(perm)
         inv[perm] = torch.arange(256, device=dev)
-        for layer, (x_in, qkv, msg, merged, hid_pre, hid, st, name) in zip(reversed(list(model.gnn.layers)), reversed(S.layers)):
+        for layer, (qkv, msg, rec, name) in zip(reversed(list(model.gnn.layers)), reversed(S.layers)):
             attn = layer.attn
+            x_in, merged, _, hid, _ = rec
             w0, w3 = layer.mlp[0].weight[:, :, 0], layer.mlp[3].weight[:, :, 0]
             acc(layer.mlp[3].weight, ops.gemm_dw(gx, hid))
             acc(layer.mlp[3].bias, ops.colsum(gx))
             g_hid = ops.gemm_dx(gx, w3)
-            dg, db = ops.batchnorm_train_backward(hid_pre, hid, g_hid, layer.mlp[1].weight.detach().float().contiguous(), st,
-                                                  n_pad, N)
-            acc(layer.mlp[1].weight, dg)
-            acc(layer.mlp[1].bias, db)
+            _bn_backward(rec, layer.mlp[1], g_hid, n_pad, N, acc)
             acc(layer.mlp[0].weight, ops.gemm_dw(g_hid, x_in, merged))
             acc(layer.mlp[0].bias, ops.colsum(g_hid))
             gx = ops.gemm_dx(g_hid, w0[:, :256], residual=gx)          # residual path + the x half of the concat
@@ -321,28 +326,25 @@ def _backward(model, S, grads):
         acc(enc[12].weight, ops.gemm_dw(gx, S.kenc_last_in))
         acc(enc[12].bias, ops.colsum(gx))
         g_h = ops.gemm_dx(gx, enc[12].weight[:, :, 0])
-        for i, (h_in, pre, y, st) in zip((9, 6, 3, 0), reversed(S.kenc)):
-            dg, db = ops.batchnorm_train_backward(pre, y, g_h, enc[i + 1].weight.detach().float().contiguous(), st, n_pad, N)
-            acc(enc[i + 1].weight, dg)
-            acc(enc[i + 1].bias, db)
-            g_w = ops.gemm_dw(g_h, h_in)
-            acc(enc[i].weight, g_w[:, :3] if i == 0 else g_w)
-            acc(enc[i].bias, ops.colsum(g_h))
-            if i:
-                g_h = ops.gemm_dx(g_h, enc[i].weight[:, :, 0])
+        for i, rec in zip((9, 6, 3), reversed(S.kenc[1:])):
+            g_h = _block_backward(rec, enc[i], enc[i + 1], g_h, n_pad, N, acc)
+        # the first block: 3 inputs padded to 16, no gradient w.r.t. the keypoints
+        _bn_backward(S.kenc[0], enc[1], g_h, n_pad, N, acc)
+        acc(enc[0].weight, ops.gemm_dw(g_h, S.kenc[0][0])[:, :3])
+        acc(enc[0].bias, ops.colsum(g_h))
     return G
 
 
 def _conf_backward(model, S, conf_g, g_md, G_all, acc):
-    """Backward of ConfidenceMLP (multi_view_matcher.py:39-53, 302-306) over every pair at once, on the pair-major
-    buffers the forward filled (rows r = (p B + b) N + i).  conf_g: per pair the gradient w.r.t. conf_scores
-    [B, N, 1] or None (zero).  Adds the gradients w.r.t. the gathered inputs to g_md [B, T, n_pad, 256] (m0, m1g) and
-    G_all [P B, N+1, N+1] (add), and the parameter gradients through acc.  Each pair's BatchNorms took their statistics over its own B N rows: one group
-    per pair (slot size B N)."""
+    """Backward of ConfidenceMLP (multi_view_matcher.py:39-53, 302-306) over every pair at once, on the state
+    _conf_forward kept (pair-major rows r = (p B + b) N + i, one BatchNorm group of B N rows per pair).  conf_g: per
+    pair the gradient w.r.t. conf_scores [B, N, 1] or None (zero).  Adds the gradients w.r.t. the gathered inputs to
+    g_md [B, T, n_pad, 256] (m0, m1g) and G_all [P B, N+1, N+1] (add), and the parameter gradients through acc."""
     B, T, N, n_pad, rows, g_bn = S.dims
     cm = model.conf_mlp
     P = len(S.pairs)
     sv = S.conf
+    n = B * N
     dbg = getattr(model, '_train_debug', None)      # tests: the head's gradients at its stage boundaries
     g_conf = torch.cat([(g.detach().float() if g is not None else torch.zeros(B, N, 1, device=S.dev)).reshape(-1)
                         for g in conf_g])
@@ -350,38 +352,28 @@ def _conf_backward(model, S, conf_g, g_md, G_all, acc):
     g_h, dw_last, db_last = ops.conf_tail_backward(sv['conf'], g_conf, sv['h'], cm.layers[0].weight[:, :, 0])
     acc(cm.layers[0].weight, dw_last)
     acc(cm.layers[0].bias, db_last)
-    bn_rows = B * N
+    if dbg is not None:
+        dbg['conf'] = {'g_h': g_h.clone()}
     g_x = g_pre_c0 = None
     for br, mods in (('f', cm.layers_f), ('c', cm.layers_c)):
+        rec0, rec3 = sv[br]
         g = g_h.clone() if br == 'f' else g_h         # the BatchNorm backward runs in place
-        if dbg is not None:
-            dbg.setdefault('conf', {})['g_h'] = g_h.clone()
-        dg, db = ops.batchnorm_train_backward(sv['pre_%s3' % br], sv['y_%s4' % br], g,
-                                              mods[4].weight.detach().float().contiguous(), sv['st_%s4' % br],
-                                              bn_rows, bn_rows)
-        acc(mods[4].weight, dg)
-        acc(mods[4].bias, db)
-        acc(mods[3].weight, ops.gemm_dw(g, sv['y_%s1' % br]))
-        acc(mods[3].bias, ops.colsum(g))
-        g1 = ops.gemm_dx(g, mods[3].weight[:, :, 0])
+        g1 = _block_backward(rec3, mods[3], mods[4], g, n, n, acc)
         if dbg is not None:
             dbg['conf'].update({'g_pre_%s3' % br: g.clone(), 'g_y_%s1' % br: g1.clone()})
-        dg, db = ops.batchnorm_train_backward(sv['pre_%s0' % br], sv['y_%s1' % br], g1,
-                                              mods[1].weight.detach().float().contiguous(), sv['st_%s1' % br],
-                                              bn_rows, bn_rows)
-        acc(mods[1].weight, dg)
-        acc(mods[1].bias, db)
+        dg = _bn_backward(rec0, mods[1], g1, n, n, acc)
         if dbg is not None:
             dbg['conf'].update({'g_pre_%s0' % br: g1.clone(), 'dgamma_%s1' % br: dg.clone()})
         acc(mods[0].bias, ops.colsum(g1))
         if br == 'f':
-            acc(mods[0].weight, ops.gemm_dw(g1, sv['m0'], sv['m1g']))
+            acc(mods[0].weight, ops.gemm_dw(g1, *rec0[:2]))
             g_x = ops.gemm_dx(g1, mods[0].weight[:, :, 0])                  # [rows, 512]: m0 | m1g
         else:
             g_pre_c0 = g1
-    # the gathers' transposes and the score-input layer (K = 1) (csrc/conf_train.cu)
+    # the gathers' transposes and the score-input layer (K = 1, its input `add` kept in its block's record)
+    # (csrc/conf_train.cu)
     i0 = sv['i0'].view(P, B, N)
-    dw_c0 = ops.conf_gather_backward(g_x, g_pre_c0, sv['add'], cm.layers_c[0].weight[:, 0, 0], i0,
+    dw_c0 = ops.conf_gather_backward(g_x, g_pre_c0, sv['c'][0][0], cm.layers_c[0].weight[:, 0, 0], i0,
                                      [(a, b_) for _, a, b_ in S.pairs], g_md, G_all)
     acc(cm.layers_c[0].weight, dw_c0)
 

@@ -4,8 +4,9 @@ backward (models/train_forward.py) -- with the stage kernels replaced by float64
 matcher, oracle/conf_grad.py for the two confidence-head kernels (csrc/conf_train.cu), oracle/pose.py and
 oracle/pose_grad.w8pt_conf_grad for the weighted eight-point and its backward.  Against the unmodified reference
 (tests/golden/train_pose_*.npz, oracle/make_train_pose_golden.py): losses, every parameter's gradient (conf_mlp.*
-included), the gradient at conf_scores_*, the matches and the head's running statistics.  Also: the optimiser helpers,
-the ratio ramp, the skipped step on a non-finite gradient, and the code generation of the new kernels."""
+included), the gradient at conf_scores_*, the matches and the head's running statistics.  Also: the head's forward
+over every pair at once, the optimiser helpers, the ratio ramp, the skipped step on a non-finite gradient, and the code
+generation of the new kernels."""
 import argparse
 import json
 import os
@@ -139,6 +140,31 @@ def test_conf_grad_off_keeps_conf_scores_without_graph(monkeypatch):
     model.config['conf_grad'] = True
     res = model(data)
     assert res['conf_scores_0_1'].requires_grad and not res['matching_scores0_0_1'].requires_grad
+
+
+def test_stage2_forward_runs_the_head_once_over_every_pair(monkeypatch):
+    """The stage-2 forward of a 3-view tuple extracts the matches of its 3 pairs in one call and runs each of the
+    confidence head's 4 BatchNorms once over the rows of every pair."""
+    from e2e_multi_view_matching_b200 import ops
+    _patch(monkeypatch)
+    z, case, model, data, opt = _setup('mv3_r05')
+    model.config.update(full_output=True, conf_grad=True)
+    head_stats = {id(m.running_mean) for m in model.conf_mlp.modules() if isinstance(m, torch.nn.BatchNorm1d)}
+    calls = {'extract_matches': 0, 'head_batchnorm_train': 0}
+    extract, bn = ops.extract_matches, ops.batchnorm_train
+
+    def counted_extract(*a, **k):
+        calls['extract_matches'] += 1
+        return extract(*a, **k)
+
+    def counted_bn(x, weight, bias, running_mean, *a, **k):
+        calls['head_batchnorm_train'] += id(running_mean) in head_stats
+        return bn(x, weight, bias, running_mean, *a, **k)
+    monkeypatch.setattr(ops, 'extract_matches', counted_extract)
+    monkeypatch.setattr(ops, 'batchnorm_train', counted_bn)
+    res = model(data)
+    assert all(res['conf_scores_' + k].requires_grad for k in ('0_1', '0_2', '1_2'))
+    assert calls == {'extract_matches': 1, 'head_batchnorm_train': 4}
 
 
 def test_loss_without_conf_scores_gives_stage1_gradients(monkeypatch):
