@@ -222,6 +222,11 @@ def lib():
     L.mvm_superpoint_select.argtypes = [_fp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _fp, _fp, _fp, _fp]
     L.mvm_superpoint_sample_batch.restype = C.c_int
     L.mvm_superpoint_sample_batch.argtypes = [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp, _fp]
+    L.mvm_image_prep_workspace_bytes.restype = C.c_size_t
+    L.mvm_image_prep_workspace_bytes.argtypes = [C.c_int] * 3
+    L.mvm_image_prep.restype = C.c_int
+    L.mvm_image_prep.argtypes = [_fp, C.c_int, C.c_int, C.c_int, _fp, _fp, _fp, C.c_int, C.c_int, _fp, _fp,
+                                 C.c_size_t, _fp]
     L.mvm_match_loss_forward.restype = C.c_int
     L.mvm_match_loss_forward.argtypes = [_fp, _fp, _fp, C.c_int, C.c_int, _fp, _fp, _fp]
     L.mvm_match_loss_backward.restype = C.c_int

@@ -468,6 +468,27 @@ int mvm_superpoint_select(const float* scores_nms, int batch, int height, int wi
 int mvm_superpoint_sample_batch(const float* dense_desc, const float* keypoints, const int* counts, int batch,
                                 int max_keypoints, int h, int w, float* descriptors, void* stream);
 
+/* ---- training-image preparation (datasets/matching_dataset.py:182-211) ------------------------------------------ */
+
+/* Bytes of the workspace mvm_image_prep needs with jitter (per-CTA fp64 partial sums of the contrast mean). */
+size_t mvm_image_prep_workspace_bytes(int n, int out_h, int out_w);
+
+/* MatchingDataset.__getitem__'s per-image transforms for a batch, without host synchronisation (graph capturable):
+ * rgb [n, src_h, src_w, 3] uint8 (decoded RGB, one source size per call) -> out [n, 1, out_h, out_w] float32 in [0, 1],
+ * the grayscale image SuperPoint takes.  Per image, in device arrays:
+ *   geometry [n, 6] int32: crop top, left, height, width inside the source, then zero rows padded above and below;
+ *   jitter_order [n, 4] int32: a permutation of 0-3 (0 brightness, 1 contrast, 2 saturation, 3 hue), and
+ *   jitter_factors [n, 4] float64: brightness, contrast, saturation, hue as the Python floats the reference passes.
+ * Both jitter arrays NULL: no jitter.  The sequence and rounding are the float32 torch / torchvision ops': ToTensor
+ * (x / 255), crop, pad, a bilinear resize (align_corners=False, no antialiasing, scale in / out) when the padded crop's
+ * size differs from the output size, the four adjustments in the given order (_blend, _rgb2hsv / _hsv2rgb), and
+ * rgb_to_grayscale.  One launch without jitter, two with (the contrast mean, deterministic, no atomics).
+ * The factor ranges and the crop windows are the caller's to check (they live on the device); an image whose
+ * geometry leaves the source or whose order is not a permutation comes out as NaN, and no load leaves its image. */
+int mvm_image_prep(const unsigned char* rgb, int n, int src_h, int src_w, const int* geometry, const int* jitter_order,
+                   const double* jitter_factors, int out_h, int out_w, float* out, void* workspace,
+                   size_t workspace_bytes, void* stream);
+
 /* ---- training path (SURVEY.md §8 a20 / f-2): losses, ground-truth matches, train-mode BatchNorm, backward kernels ---- */
 
 /* compute_match_loss (helpers.py:228-241): weighted NLL of the ground-truth assignment on the log-couplings.
