@@ -41,8 +41,12 @@ __global__ void bn_apply_kernel(const float* x, float* y, int rows, int C, int l
   const double mean_s = sums[c] / n;                                    // mean of (x - shift)
   const double var = fmax(sums[C + c] / n - mean_s * mean_s, 0.0);      // biased
   const double mean = mean_s + sh;
-  const float scale = (float)((double)gamma[c] / sqrt(var + (double)eps));
-  const float bias = (float)((double)beta[c] - mean * (double)scale);
+  const double scale_d = (double)gamma[c] / sqrt(var + (double)eps);
+  const float scale = (float)scale_d;
+  // y = (x - mean_hi) scale + (beta - mean_lo scale): x - mean_hi is exact near the mean, so a channel whose mean is
+  // large against its spread (or constant) keeps its bits; x scale + (beta - mean scale) lost ~ulp(mean scale) of them
+  const float mean_hi = (float)mean;
+  const float bias = (float)((double)beta[c] - (mean - (double)mean_hi) * scale_d);
   if (blockIdx.x == 0 && save_stats != nullptr) { save_stats[c] = (float)mean; save_stats[C + c] = (float)(1.0 / sqrt(var + (double)eps)); }
   if (blockIdx.x == 0 && running_mean != nullptr) {
     running_mean[c] = (float)((1.0 - momentum) * (double)running_mean[c] + momentum * mean);
@@ -53,7 +57,7 @@ __global__ void bn_apply_kernel(const float* x, float* y, int rows, int C, int l
   const int r0 = blockIdx.x * rows_per_block, r1 = min(rows, r0 + rows_per_block);
   for (int r = r0; r < r1; ++r) {
     if (r % n_pad >= n_valid || (r / n_pad) % slot_mod != slot_rem) continue;
-    float o = fmaf(x[(long long)r * ld + c], scale, bias);
+    float o = fmaf(x[(long long)r * ld + c] - mean_hi, scale, bias);
     if (relu) o = fmaxf(o, 0.f);
     y[(long long)r * ld + c] = o;
   }

@@ -20,7 +20,7 @@ def _ref_match_loss(log_p, gt_indices, gt_weights):
     return (torch.dot(l0, mw0.reshape(bs * ft)) + torch.dot(l1, mw1.reshape(bs * ft))) / bs
 
 
-@pytest.mark.parametrize('bs,ft', [(1, 9), (3, 65), (2, 257)])
+@pytest.mark.parametrize('bs,ft', [(1, 9), (3, 65), (2, 257), (1, 2), (2, 401), (80, 401), (1, 1025), (1, 2049)])
 def test_match_loss_forward_backward(bs, ft):
     from e2e_multi_view_matching_b200.training import compute_match_loss
     g = torch.Generator().manual_seed(ft)
