@@ -119,6 +119,9 @@ def lib():
     L.mvm_pack_views.restype = C.c_int
     L.mvm_pack_views.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
                                  C.c_int, C.c_int, C.c_int, _fp, _fp, _fp, _fp]
+    L.mvm_pack_views_ragged.restype = C.c_int
+    L.mvm_pack_views_ragged.argtypes = [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                        C.POINTER(C.c_int), _fp, C.c_int, C.c_int, C.c_int, _fp, _fp, _fp, _fp]
     L.mvm_matcher_options_default.restype = None
     L.mvm_matcher_options_default.argtypes = [C.POINTER(MatcherOptions)]
     L.mvm_matcher_forward_ex.restype = C.c_int
@@ -129,6 +132,11 @@ def lib():
     L.mvm_matcher_forward_views.restype = C.c_int
     L.mvm_matcher_forward_views.argtypes = [
         C.POINTER(MatcherWeights), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), _fp, _fp, _fp,
+        C.POINTER(C.c_float), C.c_int, C.c_float, C.POINTER(PairIO), C.c_int, _fp, C.c_size_t,
+        C.POINTER(MatcherOptions), _fp]
+    L.mvm_matcher_forward_ragged.restype = C.c_int
+    L.mvm_matcher_forward_ragged.argtypes = [
+        C.POINTER(MatcherWeights), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), _fp, _fp, _fp, _fp,
         C.POINTER(C.c_float), C.c_int, C.c_float, C.POINTER(PairIO), C.c_int, _fp, C.c_size_t,
         C.POINTER(MatcherOptions), _fp]
     for name in ('mvm_debug_set_score_kernel', 'mvm_debug_set_gemm_tile', 'mvm_debug_set_gemm_kernel',
@@ -189,6 +197,9 @@ def lib():
     L.mvm_gather_matches.restype = C.c_int
     L.mvm_gather_matches.argtypes = [_fp, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(PairIO), C.c_int,
                                      C.c_int, C.c_float, _fp, _fp, _fp, _fp, _fp]
+    L.mvm_gather_matches_ragged.restype = C.c_int
+    L.mvm_gather_matches_ragged.argtypes = [_fp, C.c_int, C.c_int, C.POINTER(C.c_int), _fp, C.POINTER(PairIO), C.c_int,
+                                            C.c_int, C.c_float, _fp, _fp, _fp, _fp, _fp]
     L.mvm_spanning_tree_init.restype = C.c_int
     L.mvm_spanning_tree_init.argtypes = [C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.c_int, C.c_int,
                                          _fp, _fp, _fp, _fp, _fp, _fp]

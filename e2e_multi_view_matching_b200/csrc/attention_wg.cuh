@@ -127,7 +127,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   const int v = blockIdx.z;
   const int T = g.segs.n_views;
   const int t = v % T, b = v / T;
-  if (q0 >= g.segs.counts[t]) return;
+  if (q0 >= slot_count(g.segs.slot, b, T, t, g.segs.counts[t])) return;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < ST; ++i) {
@@ -147,7 +147,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
       int j = 0;
       for (int sg = 0; sg < T; ++sg) {
         if (g.is_cross ? (sg == t) : (sg != t)) continue;
-        const int cnt = g.segs.counts[sg];
+        const int cnt = slot_count(g.segs.slot, b, T, sg, g.segs.counts[sg]);
         for (int k0 = 0; k0 < cnt; k0 += BKV, ++j) {
           const int s = j % ST;
           const uint32_t ph = ((j / ST) & 1) ^ 1;
@@ -423,7 +423,7 @@ attention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   int j = 0;
   for (int sg = 0; sg < T; ++sg) {
     if (g.is_cross ? (sg == t) : (sg != t)) continue;
-    const int cnt = g.segs.counts[sg];
+    const int cnt = slot_count(g.segs.slot, b, T, sg, g.segs.counts[sg]);
     for (int k0 = 0; k0 < cnt; k0 += BKV, ++j) {
       const int nvalid = cnt - k0;      // keys of this tile that exist
       const int s = j % ST;

@@ -14,7 +14,9 @@ __global__ void __launch_bounds__(256) conf_gather_kernel(const float* __restric
                                                           float* __restrict__ sc) {
   const int prob = blockIdx.y;
   const int p = prob / batch, bi = prob % batch;
-  const int m = tab.m[p], n = tab.n[p];
+  const int mc = tab.m[p], nc = tab.n[p];      // capacities: the strides of matches_a and scores
+  const int m = slot_count(tab.slot, bi, tab.n_views, tab.a[p], mc);
+  const int n = slot_count(tab.slot, bi, tab.n_views, tab.b[p], nc);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int i = blockIdx.x * 8 + warp;
   if (i >= n_pad) return;
@@ -25,9 +27,11 @@ __global__ void __launch_bounds__(256) conf_gather_kernel(const float* __restric
     if (lane == 0) sc[r] = 0.f;
     return;
   }
-  const long long idx = tab.matches_a[p][(long long)bi * m + i];
-  const int jb = idx < 0 ? n - 1 : (int)idx;   // python negative index -1 -> last keypoint
-  const int js = idx < 0 ? n : (int)idx;       // scores[..., -1] -> dustbin column
+  const long long idx = tab.matches_a[p][(long long)bi * mc + i];
+  // python negative index -1 -> this tuple's last keypoint (row 0 stands in when view b has none: m rows of a
+  // tuple without keypoints in b are never valid matches)
+  const int jb = idx < 0 ? max(n - 1, 0) : (int)idx;
+  const int js = idx < 0 ? n : (int)idx;       // scores[..., -1] -> this tuple's dustbin column
   const float4* ra = reinterpret_cast<const float4*>(
       mdesc + ((long long)(bi * tab.n_views + tab.a[p]) * n_pad + i) * 256);
   const float4* rb = reinterpret_cast<const float4*>(
@@ -37,7 +41,7 @@ __global__ void __launch_bounds__(256) conf_gather_kernel(const float* __restric
     fo[64 + c] = rb[c];
   }
   if (lane == 0)
-    sc[r] = tab.scores[p][(long long)bi * (m + 1) * (n + 1) + (long long)i * (n + 1) + js];
+    sc[r] = tab.scores[p][(long long)bi * (mc + 1) * (nc + 1) + (long long)i * (nc + 1) + js];
 }
 
 __global__ void conf_c0_kernel(const float* __restrict__ sc, const float* __restrict__ w,
@@ -55,15 +59,19 @@ __global__ void __launch_bounds__(256) conf_final_kernel(const float* __restrict
                                                          PairTable tab, int batch, int n_pad) {
   const int prob = blockIdx.y;
   const int p = prob / batch, bi = prob % batch;
-  const int m = tab.m[p];
+  const int mc = tab.m[p], m = slot_count(tab.slot, bi, tab.n_views, tab.a[p], mc);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int i = blockIdx.x * 8 + warp;
-  if (i >= m) return;
+  if (i >= mc) return;
+  if (i >= m) {                                // past this tuple's count
+    if (lane == 0) tab.conf[p][(long long)bi * mc + i] = 0.f;
+    return;
+  }
   const float* hr = h + ((long long)prob * n_pad + i) * 256;
   float acc = 0.f;
   for (int c = lane; c < 256; c += 32) acc = fmaf(hr[c], wl[c], acc);
   acc = warp_sum(acc);
-  if (lane == 0) tab.conf[p][(long long)bi * m + i] = 1.f / (1.f + expf(-(acc + bl)));
+  if (lane == 0) tab.conf[p][(long long)bi * mc + i] = 1.f / (1.f + expf(-(acc + bl)));
 }
 
 }  // namespace

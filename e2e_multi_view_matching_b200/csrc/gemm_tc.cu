@@ -106,6 +106,7 @@ struct ScoreTab {
   int n_pairs, batch, n_views, n_pad;
   int a[MVM_MAX_PAIRS], b[MVM_MAX_PAIRS], m[MVM_MAX_PAIRS], n[MVM_MAX_PAIRS];
   float* scores[MVM_MAX_PAIRS];
+  const int* slot;             // PairTable::slot (m / n are then the capacities)
 };
 
 // rn_tf32 of a finite value (ties away, == cvt.rna.tf32.f32) in two integer instructions
@@ -465,17 +466,19 @@ gemm_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (SCORE) {
       // rows of the coupling buffer are n+1 floats long: plain stores inside the [m, n] block
       const int p = prob / st.batch, bi = prob % st.batch;
-      const int pm = st.m[p], pn = st.n[p];
+      const int pm = st.m[p], pn = st.n[p];                     // capacities: the buffer's shape
+      const int em = slot_count(st.slot, bi, st.n_views, st.a[p], pm);      // this tuple's [em, en] block
+      const int en = slot_count(st.slot, bi, st.n_views, st.b[p], pn);
       float* Cp = st.scores[p] + (long long)bi * (pm + 1) * (pn + 1);
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int gm = m0 + row0 + 8 * hh;
-        if (gm >= pm) continue;
+        if (gm >= em) continue;
 #pragma unroll
         for (int i = 0; i < BN / 8; ++i) {
           const int gn = n0 + 8 * i + 2 * tq;
-          if (gn < pn) Cp[(long long)gm * (pn + 1) + gn] = g.alpha * acc[4 * i + 2 * hh];
-          if (gn + 1 < pn) Cp[(long long)gm * (pn + 1) + gn + 1] = g.alpha * acc[4 * i + 2 * hh + 1];
+          if (gn < en) Cp[(long long)gm * (pn + 1) + gn] = g.alpha * acc[4 * i + 2 * hh];
+          if (gn + 1 < en) Cp[(long long)gm * (pn + 1) + gn + 1] = g.alpha * acc[4 * i + 2 * hh + 1];
         }
       }
       continue;
@@ -842,6 +845,7 @@ int launch_score_gemm_tc(const float* mdesc, float* hi, float* lo, int n_pad, co
   const CUtensorMap* tWhi = mvm_get_tmap_2d(hi, rows, 256, 256, 128);
   const CUtensorMap* tWlo = mvm_get_tmap_2d(lo, rows, 256, 256, 128);
   ScoreTab st = no_scores();
+  st.slot = tab.slot;
   st.n_pairs = tab.n_pairs; st.batch = batch; st.n_views = tab.n_views; st.n_pad = n_pad;
   int max_m = 0, max_n = 0;
   for (int p = 0; p < tab.n_pairs; ++p) {

@@ -19,6 +19,9 @@ struct PairTable {
   float* ms_b[MVM_MAX_PAIRS];
   float* conf[MVM_MAX_PAIRS];               // [batch, m] (or nullptr)
   long long ws_off[MVM_MAX_PAIRS];          // float offset of this pair's (u,v) scratch
+  // ragged batches (mvm_matcher_forward_ragged): device [batch * n_views] true count of every view slot; m / n above are
+  // then the capacities, which set every stride.  nullptr: every slot holds exactly m / n keypoints.
+  const int* slot = nullptr;
 };
 typedef PairTable SinkhornTable;
 
@@ -81,7 +84,14 @@ int launch_score_gemm_tc(const float* mdesc, float* hi, float* lo, int n_pad, co
 struct AttnSegs {
   int n_views;
   int counts[8];
+  const int* slot = nullptr;   // as PairTable::slot: counts[] are then the capacities
 };
+
+// Keypoints of view t of tuple b: the capacity `cap` without device counts, else slot[b * n_views + t] clamped to
+// [0, cap], so that no count a caller passes can move an access outside the capacity-sized buffers.
+__device__ __forceinline__ int slot_count(const int* slot, int b, int n_views, int t, int cap) {
+  return slot ? min(max(__ldg(slot + b * n_views + t), 0), cap) : cap;
+}
 // What every attention launch needs of its segments, checked on the host before any CUDA call: 1..8 views, cross
 // attention over at least two, every count in [0, n_pad] (a larger count walks the key loop into the next view's rows),
 // and a source key for every query view that has a query row (without one the softmax denominator is 0: NaN output)

@@ -23,8 +23,10 @@ __global__ void __launch_bounds__(256) rowcol_argmax_kernel(PairTable tab, int b
                                                             float* __restrict__ max_ws) {
   const int prob = blockIdx.y;
   const int p = prob / batch, bi = prob % batch;
-  const int m = tab.m[p], n = tab.n[p], ld = n + 1;
-  const float* Z = tab.scores[p] + (long long)bi * (m + 1) * ld;
+  const int ld = tab.n[p] + 1;
+  const int m = slot_count(tab.slot, bi, tab.n_views, tab.a[p], tab.m[p]);
+  const int n = slot_count(tab.slot, bi, tab.n_views, tab.b[p], tab.n[p]);
+  const float* Z = tab.scores[p] + (long long)bi * (tab.m[p] + 1) * ld;
   int* idx0 = idx_ws + (long long)prob * 2 * n_pad;
   int* idx1 = idx0 + n_pad;
   float* max0 = max_ws + (long long)prob * n_pad;
@@ -65,18 +67,30 @@ __global__ void __launch_bounds__(256) mutual_kernel(PairTable tab, int batch, i
                                                      const float* __restrict__ max_ws) {
   const int prob = blockIdx.y;
   const int p = prob / batch, bi = prob % batch;
-  const int m = tab.m[p], n = tab.n[p];
+  const int mc = tab.m[p], nc = tab.n[p];      // capacities: the row strides of the outputs
+  const int m = slot_count(tab.slot, bi, tab.n_views, tab.a[p], mc);
+  const int n = slot_count(tab.slot, bi, tab.n_views, tab.b[p], nc);
   const int* idx0 = idx_ws + (long long)prob * 2 * n_pad;
   const int* idx1 = idx0 + n_pad;
   const float* max0 = max_ws + (long long)prob * n_pad;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  // keypoints past this tuple's counts: no match
+  if (t >= m && t < mc) { tab.matches_a[p][(long long)bi * mc + t] = -1; tab.ms_a[p][(long long)bi * mc + t] = 0.f; }
+  if (t >= n && t < nc) { tab.matches_b[p][(long long)bi * nc + t] = -1; tab.ms_b[p][(long long)bi * nc + t] = 0.f; }
+  if (m == 0 || n == 0) {
+    // one view of this tuple has no keypoints: nothing to match, and the argmax pass wrote no index of the other side
+    // (the indices below would be read from an earlier call's workspace)
+    if (t < m) { tab.matches_a[p][(long long)bi * mc + t] = -1; tab.ms_a[p][(long long)bi * mc + t] = 0.f; }
+    if (t < n) { tab.matches_b[p][(long long)bi * nc + t] = -1; tab.ms_b[p][(long long)bi * nc + t] = 0.f; }
+    return;
+  }
   if (t < m) {
     const int j = idx0[t];
     const bool mutual = idx1[j] == t;
     const float ms = mutual ? expf(max0[t]) : 0.f;
     const bool valid = mutual && (ms > thresh);
-    tab.matches_a[p][(long long)bi * m + t] = valid ? (int64_t)j : (int64_t)-1;
-    tab.ms_a[p][(long long)bi * m + t] = ms;
+    tab.matches_a[p][(long long)bi * mc + t] = valid ? (int64_t)j : (int64_t)-1;
+    tab.ms_a[p][(long long)bi * mc + t] = ms;
   }
   if (t < n) {
     const int i = idx1[t];
@@ -87,8 +101,8 @@ __global__ void __launch_bounds__(256) mutual_kernel(PairTable tab, int batch, i
     const bool valid0_i = mutual0_i && (ms0_i > thresh);
     const float ms1 = mutual1 ? ms0_i : 0.f;
     const bool valid1 = mutual1 && valid0_i;
-    tab.matches_b[p][(long long)bi * n + t] = valid1 ? (int64_t)i : (int64_t)-1;
-    tab.ms_b[p][(long long)bi * n + t] = ms1;
+    tab.matches_b[p][(long long)bi * nc + t] = valid1 ? (int64_t)i : (int64_t)-1;
+    tab.ms_b[p][(long long)bi * nc + t] = ms1;
   }
 }
 

@@ -194,11 +194,22 @@ int mvm_matcher_forward_views(const mvm_matcher_weights* w, int batch, int n_vie
                               const float* desc, const float* view_wh, int sinkhorn_iters,
                               float match_threshold, const mvm_pair_io* pairs, int n_pairs,
                               void* workspace, size_t workspace_bytes, const mvm_matcher_options* opt, void* stream_) {
+  return mvm_matcher_forward_ragged(w, batch, n_views, n_pad, counts, nullptr, kpts, kscores, desc, view_wh, sinkhorn_iters,
+                                    match_threshold, pairs, n_pairs, workspace, workspace_bytes, opt, stream_);
+}
+
+int mvm_matcher_forward_ragged(const mvm_matcher_weights* w, int batch, int n_views, int n_pad,
+                               const int* counts, const int* slot_counts, const float* kpts, const float* kscores,
+                               const float* desc, const float* view_wh, int sinkhorn_iters,
+                               float match_threshold, const mvm_pair_io* pairs, int n_pairs,
+                               void* workspace, size_t workspace_bytes, const mvm_matcher_options* opt, void* stream_) {
   cudaStream_t s = (cudaStream_t)stream_;
   mvm_matcher_options o;
   if (opt) o = *opt; else mvm_matcher_options_default(&o);
   MVM_REQUIRE(o.math_mode == 0 || o.math_mode == 1 || o.math_mode == 3);
   MVM_REQUIRE(o.sinkhorn_variant >= 0 && o.sinkhorn_variant <= 4);
+  // device counts reach the tensor-core kernels of math mode 3 only (the SIMT attention and score kernels keep host counts)
+  MVM_REQUIRE(!slot_counts || (o.math_mode == 3 && o.score_kernel));
   MVM_REQUIRE(w && counts && kpts && kscores && desc && view_wh && pairs && workspace && sinkhorn_iters >= 1);
   MVM_REQUIRE(batch >= 1 && n_views >= 2 && n_views <= MVM_MAX_VIEWS);
   MVM_REQUIRE(n_pad >= 64 && n_pad % 64 == 0);
@@ -223,6 +234,7 @@ int mvm_matcher_forward_views(const mvm_matcher_weights* w, int batch, int n_vie
   AttnSegs segs;
   segs.n_views = n_views;
   for (int t = 0; t < 8; ++t) segs.counts[t] = t < n_views ? counts[t] : 0;
+  segs.slot = slot_counts;
 
   // keypoint encoder + descriptor add (multi_view_matcher.py:265-269)
   MVM_TRY(launch_transpose_cn(desc, ws.DT, V, 256, n_pad, s));
@@ -284,6 +296,7 @@ int mvm_matcher_forward_views(const mvm_matcher_weights* w, int batch, int n_vie
 
   PairTable tab;
   MVM_TRY(fill_pair_table(tab, pairs, n_pairs, n_views, counts, batch));
+  tab.slot = slot_counts;
   // score matrices: tensor cores in the 3xTF32 mode (the K_lo / V^T_lo planes of the GNN are free again and
   // hold the tf32 planes of the descriptors), fp32 CUDA cores otherwise
   if (cx.math_mode == 3 && cx.score_tc) MVM_TRY(launch_score_gemm_tc(ws.MD, ws.KLO, ws.VTLO, n_pad, tab, batch, 1.0f / 16.0f, s));

@@ -43,9 +43,9 @@ __global__ void __launch_bounds__(NT) gather_matches_kernel(const float* __restr
   __shared__ int s_base;
   const int prob = blockIdx.x;                  // = bi * n_pairs + p
   const int bi = prob / tab.n_pairs, p = prob % tab.n_pairs;
-  const int m = tab.m[p];
-  const int64_t* ma = tab.matches_a[p] + (long long)bi * m;
-  const float* cf = tab.conf[p] + (long long)bi * m;
+  const int m = slot_count(tab.slot, bi, tab.n_views, tab.a[p], tab.m[p]);
+  const int64_t* ma = tab.matches_a[p] + (long long)bi * tab.m[p];      // capacity strides
+  const float* cf = tab.conf[p] + (long long)bi * tab.m[p];
   const float* ka = kpts + (long long)(bi * tab.n_views + tab.a[p]) * n_pad * 2;
   const float* kb = kpts + (long long)(bi * tab.n_views + tab.b[p]) * n_pad * 2;
   float* o0 = mk0 + (long long)prob * n_pad * 2;
@@ -840,12 +840,22 @@ extern "C" {
 int mvm_gather_matches(const float* kpts, int n_views, int n_pad, const int* counts,
                        const mvm_pair_io* pairs, int n_pairs, int batch, float conf_thresh,
                        float* mkpts_a, float* mkpts_b, float* mconf, int* n_valid, void* stream) {
+  return mvm_gather_matches_ragged(kpts, n_views, n_pad, counts, nullptr, pairs, n_pairs, batch, conf_thresh, mkpts_a,
+                                   mkpts_b, mconf, n_valid, stream);
+}
+
+int mvm_gather_matches_ragged(const float* kpts, int n_views, int n_pad, const int* counts, const int* slot_counts,
+                              const mvm_pair_io* pairs, int n_pairs, int batch, float conf_thresh,
+                              float* mkpts_a, float* mkpts_b, float* mconf, int* n_valid, void* stream) {
   MVM_REQUIRE(kpts && counts && pairs && mkpts_a && mkpts_b && mconf && n_valid);
   MVM_REQUIRE(n_pairs >= 1 && n_pairs <= MVM_MAX_PAIRS && batch >= 1);
   MvmProfScope prof__(MVM_TAG_MISC, (cudaStream_t)stream);
   PairTable tab;
-  tab.n_pairs = n_pairs; tab.n_views = n_views;
+  tab.n_pairs = n_pairs; tab.n_views = n_views; tab.slot = slot_counts;
   for (int p = 0; p < n_pairs; ++p) {
+    // the slot of a view indexes slot_counts
+    MVM_REQUIRE(!slot_counts || (pairs[p].view_a >= 0 && pairs[p].view_a < n_views && pairs[p].view_b >= 0 &&
+                                 pairs[p].view_b < n_views));
     tab.a[p] = pairs[p].view_a; tab.b[p] = pairs[p].view_b;
     tab.m[p] = counts[pairs[p].view_a]; tab.n[p] = counts[pairs[p].view_b];
     tab.matches_a[p] = pairs[p].matches_a; tab.conf[p] = pairs[p].conf;

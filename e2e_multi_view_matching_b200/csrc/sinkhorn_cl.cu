@@ -176,9 +176,11 @@ __global__ void __launch_bounds__(1024 / RG, 1) sinkhorn_cl_kernel(PairTable tab
   const float alpha = cfg.alpha;
 
   const int p = prob / cfg.batch, bi = prob % cfg.batch;
-  const int m = tab.m[p], n = tab.n[p];
-  const int ld = n + 1;
-  float* Zg = tab.scores[p] + (long long)bi * (m + 1) * ld;
+  // this problem's counts; the buffer keeps the capacity shape [m_cap + 1, n_cap + 1] (PairTable::slot)
+  const int m = slot_count(tab.slot, bi, tab.n_views, tab.a[p], tab.m[p]);
+  const int n = slot_count(tab.slot, bi, tab.n_views, tab.b[p], tab.n[p]);
+  const int ld = tab.n[p] + 1;
+  float* Zg = tab.scores[p] + (long long)bi * (tab.m[p] + 1) * ld;
   const int R = (m + C - 1) / C;
   const int r0 = min(m, (int)c * R), nrows = min(m, r0 + R) - r0;
   constexpr int LD = CL_MAXN;

@@ -62,9 +62,11 @@ __global__ void __launch_bounds__(1024, 1) sinkhorn_exp_kernel(PairTable tab, Si
 
   for (int prob = group; prob < n_prob; prob += cfg.NG) {
     const int p = prob / cfg.batch, bi = prob % cfg.batch;
-    const int m = tab.m[p], n = tab.n[p];
-    const int ld = n + 1;
-    float* Zg = tab.scores[p] + (long long)bi * (m + 1) * ld;
+    // this problem's counts; the buffer keeps the capacity shape [m_cap + 1, n_cap + 1] (PairTable::slot)
+    const int m = slot_count(tab.slot, bi, tab.n_views, tab.a[p], tab.m[p]);
+    const int n = slot_count(tab.slot, bi, tab.n_views, tab.b[p], tab.n[p]);
+    const int ld = tab.n[p] + 1;
+    float* Zg = tab.scores[p] + (long long)bi * (tab.m[p] + 1) * ld;
     const int R = (m + G - 1) / G;
     const int r0 = min(m, c * R), r1 = min(m, r0 + R);
     const int nrows = r1 - r0;

@@ -9,8 +9,9 @@ With --images the tuples are image-in, as in the reference: the scene is rendere
 (synthetic.render_tuple_images) and SuperPoint (seeded weights, or a superpoint_v1.pth-style state dict given with
 --superpoint_weights; max_keypoints, keypoint_threshold, nms_radius and remove_borders as eval_multi_view.py:125-141)
 finds the keypoints on the device before the matcher (run_super_point, eval_multi_view.py:157), one tuple per batch as
-the reference's test loader (batch_size=1), so every view keeps its own keypoint count.  Without it, the matcher gets
-the synthetic keypoints directly.
+the reference's test loader (batch_size=1), so every view keeps its own keypoint count.  --image_batch N runs N tuples
+per batch instead: their views keep their own counts as a ragged batch (MultiViewPipeline.run_tuples).  Without --images, the
+matcher gets the synthetic keypoints directly.
 
     python -m e2e_multi_view_matching_b200.eval_multi_view --n_tuples 16 --out result.json
     python -m e2e_multi_view_matching_b200.eval_multi_view --images --n_tuples 16 --out result.json
@@ -51,6 +52,8 @@ def main(argv=None):
     ap.add_argument('--math_mode', type=int, default=3)
     ap.add_argument('--out', default=None)
     ap.add_argument('--images', action='store_true', help='render the tuples and run SuperPoint on them')
+    ap.add_argument('--image_batch', type=int, default=1,
+                    help='tuples per batch with --images (1: the reference test loader; more: ragged batches)')
     ap.add_argument('--superpoint_weights', default=None)
     ap.add_argument('--keypoint_threshold', type=float, default=0.005)
     ap.add_argument('--nms_radius', type=int, default=4)
@@ -84,24 +87,32 @@ def main(argv=None):
         if not opt.superpoint_weights:
             superpoint.load_state_dict({k: torch.from_numpy(v) for k, v in make_superpoint_state_dict(opt.seed).items()})
         superpoint = superpoint.cuda()
-        opt.batch = 1
+        opt.batch = opt.image_batch
     pipe = MultiViewPipeline(matcher, superpoint=superpoint)
     pose_errors = [[], [], []]
     with torch.no_grad():
         for start in range(0, opt.n_tuples, opt.batch):
             b = min(opt.batch, opt.n_tuples - start)
             if opt.images:
-                data = render_tuple_images(make_scene_tuple_inputs(1000 + start, opt.tuple_size, opt.max_keypoints,
-                                                                   batch=b, noise_px=0.0), seed=1000 + start)
-                data = {k: (torch.from_numpy(v).cuda() if isinstance(v, np.ndarray) else v) for k, v in data.items()
+                # tuple i is rendered from seed 1000 + i whatever the batch size, so --image_batch changes the batching
+                # and nothing else
+                parts = [render_tuple_images(make_scene_tuple_inputs(1000 + i, opt.tuple_size, opt.max_keypoints,
+                                                                     batch=1, noise_px=0.0), seed=1000 + i)
+                         for i in range(start, start + b)]
+                data = {k: (torch.from_numpy(np.concatenate([p[k] for p in parts])).cuda() if isinstance(v, np.ndarray)
+                            else v) for k, v in parts[0].items()
                         if not k.startswith(('keypoints', 'scores', 'descriptors'))}
             else:
                 data = make_scene_tuple_inputs(1000 + start, opt.tuple_size, opt.max_keypoints, batch=b)
                 data = {k: (torch.from_numpy(v).cuda() if isinstance(v, np.ndarray) and not k.startswith('image')
                             else (torch.empty(v.shape, device='meta') if isinstance(v, np.ndarray) else v))
                         for k, v in data.items()}
-            _, pose = pipe(data)
-            for e in MultiViewPipeline.pair_errors(data, pose, opt.tuple_size):
+            if opt.images:
+                # one (result, pose) per tuple: the SuperPoint counts of a batch may differ between tuples
+                errs = MultiViewPipeline.tuple_errors(data, [p for _, p in pipe.run_tuples(data)], opt.tuple_size)
+            else:
+                errs = MultiViewPipeline.pair_errors(data, pipe(data)[1], opt.tuple_size)
+            for e in errs:
                 for i in range(3):
                     pose_errors[i].append(e[i])
     metrics = write_result(pose_errors, opt.out)

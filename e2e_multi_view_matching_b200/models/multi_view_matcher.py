@@ -6,6 +6,7 @@ never runs them -- it repacks the weights (packing.py) and makes one C-ABI call 
 batch (mvm_matcher_forward).  Eval mode only: the training branch is SURVEY.md §8 f-2.
 """
 import ctypes as C
+import re
 
 import torch
 from torch import nn
@@ -90,9 +91,11 @@ class MatcherEngine:
             self._ws[key] = buf
         return buf
 
-    def run(self, packed, views, view_wh, pair_ids, sinkhorn_iters, match_threshold):
+    def run(self, packed, views, view_wh, pair_ids, sinkhorn_iters, match_threshold, slot_counts=None):
         """views: list (per view slot) of (kpts [B,n,2], scores [B,n], desc [B,256,n]) CUDA tensors; view_wh: list (per
         view slot) of the (width, height) its keypoints are normalised by.
+        slot_counts: None, or a [B, T] int32 CUDA tensor of the true keypoints of every (tuple, view slot) of a ragged
+        batch; n is then each view's capacity and the outputs keep the capacity shapes (mvm_matcher_forward_ragged).
         Returns {pair: dict of output tensors} following the reference's shapes/dtypes."""
         lib = _lib.lib()
         T = len(views)
@@ -110,9 +113,18 @@ class MatcherEngine:
             assert k.dtype == s.dtype == d.dtype == torch.float32 and d.shape[1] == 256
         ptrs = [(C.c_void_p * T)(*[v[i].data_ptr() for v in views]) for i in range(3)]
         cnt_pack = (C.c_int * T)(*counts)
+        if slot_counts is not None:
+            if (slot_counts.device != dev or slot_counts.dtype != torch.int32 or tuple(slot_counts.shape) != (B, T)):
+                raise _lib.MvmError('slot_counts must be a [%d, %d] int32 tensor on %s' % (B, T, dev))
+            slot_counts = slot_counts.contiguous()
         with torch.cuda.device(dev):
-            _lib.check(lib.mvm_pack_views(ptrs[0], ptrs[1], ptrs[2], cnt_pack, B, T, n_pad, _lib.ptr(kp), _lib.ptr(sc),
-                                          _lib.ptr(de), _lib.stream_ptr()), 'mvm_pack_views')
+            if slot_counts is None:
+                _lib.check(lib.mvm_pack_views(ptrs[0], ptrs[1], ptrs[2], cnt_pack, B, T, n_pad, _lib.ptr(kp),
+                                              _lib.ptr(sc), _lib.ptr(de), _lib.stream_ptr()), 'mvm_pack_views')
+            else:
+                _lib.check(lib.mvm_pack_views_ragged(ptrs[0], ptrs[1], ptrs[2], cnt_pack, _lib.ptr(slot_counts), B, T,
+                                                     n_pad, _lib.ptr(kp), _lib.ptr(sc), _lib.ptr(de), _lib.stream_ptr()),
+                           'mvm_pack_views_ragged')
         n_pairs = len(pair_ids)
         pairs = (_lib.PairIO * n_pairs)()
         outs = {}
@@ -140,7 +152,13 @@ class MatcherEngine:
         cnt = (C.c_int * T)(*counts)
         wh = [(float(w), float(h)) for w, h in view_wh]
         with torch.cuda.device(dev):
-            if len(set(wh)) == 1:
+            if slot_counts is not None:
+                table = (C.c_float * (2 * T))(*[x for pair in wh for x in pair])
+                rc = lib.mvm_matcher_forward_ragged(
+                    C.byref(packed.struct), B, T, n_pad, cnt, _lib.ptr(slot_counts), _lib.ptr(kp), _lib.ptr(sc),
+                    _lib.ptr(de), table, int(sinkhorn_iters), float(match_threshold),
+                    pairs, n_pairs, _lib.ptr(ws), nbytes, None, _lib.stream_ptr())
+            elif len(set(wh)) == 1:
                 # one image size for every view: the plain entry point (the same arithmetic, bit for bit)
                 rc = lib.mvm_matcher_forward(
                     C.byref(packed.struct), B, T, n_pad, cnt, _lib.ptr(kp), _lib.ptr(sc), _lib.ptr(de),
@@ -155,8 +173,52 @@ class MatcherEngine:
         _lib.check(rc, 'mvm_matcher_forward')
         # device-resident state the pose stage continues from (no host round trip)
         self.last = {'kpts': kp, 'counts': counts, 'n_pad': n_pad, 'pairs': pairs, 'pair_ids': list(pair_ids),
-                     'outs': outs, 'batch': B, 'n_views': T}
+                     'outs': outs, 'batch': B, 'n_views': T, 'slot_counts': slot_counts}
         return outs
+
+
+def slot_counts_of(data, view_ids):
+    """[B, len(view_ids)] int32 device counts of a ragged batch (data['counts{i}'], [B] each, as SuperPoint.forward_batch
+    names them), or None when `data` carries no counts (every tuple fills its tensors)."""
+    if 'counts%d' % view_ids[0] not in data:
+        return None
+    return torch.stack([data['counts%d' % i].to(torch.int32) for i in view_ids], 1).contiguous()
+
+
+# matches{x}_{a}_{b}, matching_scores{x}_{a}_{b}, scores_{a}_{b}, conf_scores_{a}_{b}, keypoints{i}, scores{i}, descriptors{i}
+_RAGGED_KEY = re.compile(r'(matches|matching_scores|scores_|conf_scores_|keypoints|scores|descriptors)(\d+)(?:_\d+_\d+|_(\d+))?')
+
+
+def split_ragged_result(result, counts):
+    """Cuts the padded outputs of a ragged batch into one dict per tuple with the shapes a batch-of-one call returns.
+    counts: per view id, the [B] keypoint counts (tensors or lists; read to the host once).  Keys handled: the matcher's
+    matches* / matching_scores* / scores_* / conf_scores_*, and keypoints* / scores* / descriptors* of the front end;
+    counts* are dropped, other entries are sliced along the batch only."""
+    cnt = torch.stack([torch.as_tensor(c, dtype=torch.int64).cpu() for c in counts], 1).tolist()   # [B][T]
+    out = []
+    for nb in cnt:
+        b = len(out)
+        d = {}
+        for k, v in result.items():
+            m = _RAGGED_KEY.fullmatch(k)
+            if k.startswith('counts') or v is None:
+                continue
+            if m is None:
+                d[k] = v[b:b + 1] if torch.is_tensor(v) else v
+                continue
+            name, i0 = m.group(1), int(m.group(2))
+            if name in ('matches', 'matching_scores'):          # matches{x}_{a}_{b}: one entry per keypoint of view x
+                d[k] = v[b:b + 1, :nb[i0]]
+            elif name == 'scores_':                              # scores_{a}_{b}: coupling block with its dustbins
+                d[k] = v[b:b + 1, :nb[i0] + 1, :nb[int(m.group(3))] + 1]
+            elif name == 'conf_scores_':
+                d[k] = v[b:b + 1, :nb[i0]]
+            elif name == 'descriptors':
+                d[k] = v[b:b + 1, :, :nb[i0]]
+            else:                                                # keypoints{i}, scores{i}
+                d[k] = v[b:b + 1, :nb[i0]]
+        out.append(d)
+    return out
 
 
 class MultiViewMatcher(nn.Module):
@@ -232,6 +294,9 @@ class MultiViewMatcher(nn.Module):
                 data['descriptors' + str(i)].float())
 
     def forward(self, data):
+        """The reference's forward.  A ragged batch carries counts{i} ([B] int32 CUDA tensors, SuperPoint.forward_batch's
+        name) next to keypoints{i} [B, n_i, 2] & co., whose width n_i is then a capacity: the outputs keep the capacity
+        shapes, tuple b's entries are the top-left blocks of its counts (split_ragged_result cuts them apart)."""
         if self.training:
             # batch-statistics BatchNorm cannot be folded into the packed weights: the train branch sequences the stage
             # kernels (models/train_forward.py); with autograd enabled the `scores_*` outputs carry the graph of
@@ -264,7 +329,7 @@ class MultiViewMatcher(nn.Module):
                         # each view normalised by its own image (multi_view_matcher.py:165-166)
                         outs = self._engine.run(packed, [self._view(data, id0), self._view(data, id1)],
                                                 [image_wh(data, id0), image_wh(data, id1)], [(0, 1)], iters,
-                                                self.match_threshold)
+                                                self.match_threshold, slot_counts_of(data, [id0, id1]))
                         self._engine.last['view_ids'] = [id0, id1]
                         self._publish(result, outs, {0: id0, 1: id1})
                 return result
@@ -280,7 +345,7 @@ class MultiViewMatcher(nn.Module):
                 slot = {i: s for s, i in enumerate(with_kpts)}
                 pair_ids = [(slot[i0], slot[i1]) for i1 in with_kpts for i0 in with_kpts if i0 < i1]
                 outs = self._engine.run(packed, [self._view(data, i) for i in with_kpts], [wh] * len(with_kpts),
-                                        pair_ids, iters, self.match_threshold)
+                                        pair_ids, iters, self.match_threshold, slot_counts_of(data, with_kpts))
                 self._engine.last['view_ids'] = list(with_kpts)     # slot -> view id of the caller's data dict
                 self._publish(result, outs, {s: i for i, s in slot.items()})
         return result

@@ -7,7 +7,7 @@ from torch import nn
 
 from .. import _lib
 from ..packing import PackedMatcher
-from .multi_view_matcher import KeypointEncoder, AttentionalGNN, MatcherEngine, image_wh
+from .multi_view_matcher import KeypointEncoder, AttentionalGNN, MatcherEngine, image_wh, slot_counts_of
 
 
 class SuperGlue(nn.Module):
@@ -65,7 +65,8 @@ class SuperGlue(nn.Module):
         with torch.no_grad():
             # each view normalised by its own image (superglue.py:245-246)
             o = self._engine.run(packed, views, [image_wh(data, 0), image_wh(data, 1)], [(0, 1)],
-                                 self.config['sinkhorn_iterations'], self.config['match_threshold'])[(0, 1)]
+                                 self.config['sinkhorn_iterations'], self.config['match_threshold'],
+                                 slot_counts_of(data, [0, 1]))[(0, 1)]
         return {
             'matches0': o['matches_a'],
             'matches1': o['matches_b'],

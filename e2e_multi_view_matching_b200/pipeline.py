@@ -13,7 +13,8 @@ import types
 import numpy as np
 import torch
 
-from .models.multi_view_matcher import MultiViewMatcher
+from . import _lib
+from .models.multi_view_matcher import MultiViewMatcher, split_ragged_result
 from .pose_optimization.multi_view.pose_engine import MultiViewPoseEngine
 
 
@@ -59,7 +60,35 @@ class MultiViewPipeline:
         keypoints are skipped by the matcher (multi_view_matcher.py:155-162), so the pose stage works on view SLOTS:
         pose['view_ids'][s] is the id (in `data`) of slot s, the extrinsics / pair tensors are indexed by slot.  pose
         is None when fewer than two views have keypoints (nothing to estimate: the reference's "cannot compute pose"
-        case)."""
+        case).  A batch of tuples has one tensor per output, so an image batch (B > 1) whose SuperPoint counts differ
+        between tuples is refused here: run_tuples matches it as a ragged batch."""
+        out = self._run(data, global_ba)
+        if isinstance(out, list):
+            raise ValueError('the SuperPoint counts of this image batch differ between tuples: use '
+                             'MultiViewPipeline.run_tuples, which returns one (result, pose) per tuple')
+        return out
+
+    def run_tuples(self, data, global_ba=True):
+        """-> a list with one (result, pose) per tuple of the batch, each as __call__ returns it for that tuple alone
+        (batch dimension 1, tensors cut to the tuple's keypoint counts).  Any batch: keypoints given (counts{i} for a
+        ragged one), or images, whose SuperPoint counts may differ between tuples (a ragged batch, see _run_ragged)."""
+        out = self._run(data, global_ba)
+        if isinstance(out, list):
+            return out
+        result, pose = out
+        B = result['keypoints0'].shape[0] if 'keypoints0' in result else data['keypoints0'].shape[0]
+        if B == 1:
+            return [out]
+        src = result if 'keypoints0' in result else data      # the front end's features, or the caller's
+        T = len(data['ids'])
+        counts = [data['counts%d' % i] if 'counts%d' % i in data else [src['keypoints%d' % i].shape[1]] * B
+                  for i in range(T)]
+        results = split_ragged_result(result, counts)
+        return [(results[b], None if pose is None else
+                 {k: (v[b:b + 1] if torch.is_tensor(v) else v) for k, v in pose.items()}) for b in range(B)]
+
+    def _run(self, data, global_ba):
+        """__call__'s work; a list of per-tuple (result, pose) for a ragged image batch."""
         features = {}
         if 'keypoints0' not in data:
             if self.superpoint is None:
@@ -69,8 +98,13 @@ class MultiViewPipeline:
             batch = data['image0'].shape[0]
             data = dict(data)
             before = set(data)
-            run_super_point(types.SimpleNamespace(batch_size=batch), data, self.superpoint,
-                            merge=len({tuple(data[k].shape) for k in views}) == 1)
+            merge = len({tuple(data[k].shape) for k in views}) == 1
+            if batch > 1 and merge and self._batched_front_end(data):
+                ragged = self._super_point_batch(data)
+                if ragged is not None:
+                    return self._run_ragged(data, ragged, global_ba)
+            else:
+                run_super_point(types.SimpleNamespace(batch_size=batch), data, self.superpoint, merge=merge)
             features = {k: data[k] for k in set(data) - before}
         result = self.matcher(data)
         result.update(features)
@@ -82,6 +116,73 @@ class MultiViewPipeline:
         pose = self.pose.run(state, intr, global_ba=global_ba)
         pose['view_ids'] = list(view_ids)
         return result, pose
+
+    def _batched_front_end(self, data):
+        """True when SuperPoint.forward_batch serves this image batch (run_super_point's condition for it)."""
+        k_max = self.superpoint.config['max_keypoints']
+        h, w = data['image0'].shape[-2:]
+        return 0 < k_max <= min(_lib.MVM_SUPERPOINT_MAX_SELECT, (h // 8 * 8) * (w // 8 * 8))
+
+    def _super_point_batch(self, data):
+        """SuperPoint on every image of the batch in one forward_batch.  Every image at max_keypoints (always so with
+        fill_with_random_keypoints): data gets keypoints{i} / scores{i} / descriptors{i} as run_super_point gives them,
+        returns None.  Otherwise returns the [T, B] host counts and the padded [T, B, ...] device tensors."""
+        T, B = len(data['ids']), data['image0'].shape[0]
+        K = self.superpoint.config['max_keypoints']
+        out = self.superpoint.forward_batch(torch.cat([data['image%d' % i].cuda() for i in range(T)], 0))
+        counts = out['counts'].view(T, B)
+        host = counts.tolist()               # the one read of the counts per batch: routing and splitting need it
+        feats = {k: out[k].view(T, B, *out[k].shape[1:]) for k in ('keypoints', 'scores', 'descriptors')}
+        if all(n == K for row in host for n in row):
+            for k, v in feats.items():
+                for m in range(T):
+                    data[k + str(m)] = v[m]
+            return None
+        return host, counts, feats
+
+    def _run_ragged(self, data, ragged, global_ba):
+        """An image batch whose views have different keypoint counts per tuple.  The tuples with keypoints in every
+        view run as one ragged batch (counts{i} on the device, capacities = the largest count of each view); a tuple
+        with an empty view runs alone through the batch-of-one call, which drops that view as the reference does, so it
+        cannot touch another tuple's results.  Returns one (result, pose) per tuple, each shaped as a batch-of-one call
+        returns it."""
+        host, counts, feats = ragged
+        T, B = len(host), len(host[0])
+        full = [b for b in range(B) if all(host[m][b] > 0 for m in range(T))]
+        alone = [b for b in range(B) if b not in full]
+        results, poses = [None] * B, [None] * B
+        if len(full) < 2:
+            alone, full = sorted(alone + full), []
+
+        def tuples(idx, caps):
+            sel = torch.tensor(idx, device=counts.device)
+            d = {k: (v.index_select(0, sel.to(v.device)) if torch.is_tensor(v) and v.dim() > 0 and v.shape[0] == B else v)
+                 for k, v in data.items()}
+            for m in range(T):
+                d['keypoints%d' % m] = feats['keypoints'][m].index_select(0, sel)[:, :caps[m]]
+                d['scores%d' % m] = feats['scores'][m].index_select(0, sel)[:, :caps[m]]
+                d['descriptors%d' % m] = feats['descriptors'][m].index_select(0, sel)[:, :, :caps[m]]
+            return d
+
+        for b in alone:
+            d = tuples([b], [host[m][b] for m in range(T)])
+            results[b], poses[b] = self._run(d, global_ba)
+            results[b].update({k: d[k] for k in d if k.startswith(('keypoints', 'scores', 'descriptors'))})
+        if full:
+            d = tuples(full, [max(host[m][b] for b in full) for m in range(T)])
+            sel = torch.tensor(full, device=counts.device)
+            for m in range(T):
+                d['counts%d' % m] = counts[m].index_select(0, sel)
+            result = self.matcher(d)
+            result.update({k: d[k] for k in d if k.startswith(('keypoints', 'scores', 'descriptors'))})
+            state = self.matcher._engine.last
+            pose = self.pose.run(state, [d['intr%d' % i] for i in state['view_ids']], global_ba=global_ba)
+            pose['view_ids'] = list(state['view_ids'])
+            split = split_ragged_result(result, [[host[m][b] for b in full] for m in range(T)])
+            for i, b in enumerate(full):
+                results[b] = split[i]
+                poses[b] = {k: (v[i:i + 1] if torch.is_tensor(v) else v) for k, v in pose.items()}
+        return list(zip(results, poses))
 
     @staticmethod
     def pair_errors(data, pose, tuple_size):
@@ -106,6 +207,13 @@ class MultiViewPipeline:
                     et, er = compute_pose_error_np(T_gt, T_pr[:3, :3], T_pr[:3, 3])
                     errs.append((max(et, er), et, er))
         return errs
+
+    @staticmethod
+    def tuple_errors(data, poses, tuple_size):
+        """pair_errors of run_tuples' output: poses = the pose of every tuple of `data`, in order."""
+        return [e for b, p in enumerate(poses)
+                for e in MultiViewPipeline.pair_errors({'pose%d' % i: data['pose%d' % i][b:b + 1]
+                                                        for i in range(tuple_size)}, p, tuple_size)]
 
 
 class PairPipeline:

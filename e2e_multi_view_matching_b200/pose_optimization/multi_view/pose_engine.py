@@ -47,6 +47,16 @@ class MultiViewPoseEngine:
             self._pair_index_key = key
         return self._pair_index_val
 
+    def _gather(self, lib, state, mk0, mk1, mconf, n_valid, sp):
+        """Valid-match compaction of every (tuple, pair); a ragged batch (state['slot_counts']) bounds each tuple by its
+        device counts."""
+        kp, T, P, B = state['kpts'], state['n_views'], len(state['pair_ids']), state['batch']
+        cnt = (C.c_int * T)(*state['counts'])
+        _lib.check(lib.mvm_gather_matches_ragged(_lib.ptr(kp), T, state['n_pad'], cnt,
+                                                 _lib.ptr(state.get('slot_counts')), state['pairs'], P, B,
+                                                 float(self.conf_thresh), _lib.ptr(mk0), _lib.ptr(mk1), _lib.ptr(mconf),
+                                                 _lib.ptr(n_valid), sp), 'mvm_gather_matches_ragged')
+
     def run(self, state, intr, global_ba=True, rel_pose_method='w8pt_ba'):
         """state: MatcherEngine.last of the matcher call; intr: list (per view) of [B,3,3]/[B,4,4]
         intrinsics.  Returns dict with pairwise poses and (if global_ba) absolute extrinsics.
@@ -60,7 +70,7 @@ class MultiViewPoseEngine:
                                  % rel_pose_method)
             return self._run_ransac(state, intr, rel_pose_method == 'ransac_ba')
         lib = _lib.lib()
-        kp, counts, n_pad = state['kpts'], state['counts'], state['n_pad']
+        kp, n_pad = state['kpts'], state['n_pad']
         pairs, pair_ids = state['pairs'], state['pair_ids']
         B, T, P = state['batch'], state['n_views'], len(state['pair_ids'])
         dev = kp.device
@@ -69,12 +79,9 @@ class MultiViewPoseEngine:
         mk1 = torch.empty(B, P, n_pad, 2, **f32)
         mconf = torch.empty(B, P, n_pad, **f32)
         n_valid = torch.empty(B, P, dtype=torch.int32, device=dev)
-        cnt = (C.c_int * T)(*counts)
         sp = _lib.stream_ptr()
         with torch.cuda.device(dev):
-            _lib.check(lib.mvm_gather_matches(_lib.ptr(kp), T, n_pad, cnt, pairs, P, B, float(self.conf_thresh),
-                                              _lib.ptr(mk0), _lib.ptr(mk1), _lib.ptr(mconf), _lib.ptr(n_valid), sp),
-                       'mvm_gather_matches')
+            self._gather(lib, state, mk0, mk1, mconf, n_valid, sp)
             i4 = torch.stack([_intr4(k.to(dev)) for k in intr], 1)                    # [B,T,4]
             ia_idx, ib_idx = self._pair_index(pair_ids, dev)
             ia = i4.index_select(1, ia_idx)                                           # [B,P,4]
@@ -131,7 +138,7 @@ class MultiViewPoseEngine:
         """eval_pairs.py:228-243: estimate_pose (RANSAC + recoverPose) on the valid matches of every pair, then, with
         refine, the two-view BA on the inliers of that pose weighted by the raw match confidences."""
         lib = _lib.lib()
-        kp, counts, n_pad = state['kpts'], state['counts'], state['n_pad']
+        kp, n_pad = state['kpts'], state['n_pad']
         pairs, pair_ids = state['pairs'], state['pair_ids']
         B, T, P = state['batch'], state['n_views'], len(state['pair_ids'])
         dev = kp.device
@@ -143,12 +150,9 @@ class MultiViewPoseEngine:
         mk1 = torch.empty(B, P, n_pad, 2, **f32)
         mconf = torch.empty(B, P, n_pad, **f32)
         n_valid = torch.empty(B, P, **i32)
-        cnt = (C.c_int * T)(*counts)
         sp = _lib.stream_ptr()
         with torch.cuda.device(dev):
-            _lib.check(lib.mvm_gather_matches(_lib.ptr(kp), T, n_pad, cnt, pairs, P, B, float(self.conf_thresh),
-                                              _lib.ptr(mk0), _lib.ptr(mk1), _lib.ptr(mconf), _lib.ptr(n_valid), sp),
-                       'mvm_gather_matches')
+            self._gather(lib, state, mk0, mk1, mconf, n_valid, sp)
             i4 = torch.stack([_intr4(k.to(dev)) for k in intr], 1)
             ia_idx, ib_idx = self._pair_index(pair_ids, dev)
             ia = i4.index_select(1, ia_idx).contiguous()

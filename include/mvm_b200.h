@@ -91,8 +91,15 @@ typedef struct mvm_pair_io {
 int mvm_pack_views(const float* const* kpts, const float* const* scores, const float* const* desc,
                    const int* counts, int batch, int n_views, int n_pad, float* out_kpts, float* out_scores,
                    float* out_desc, void* stream);
+/* mvm_pack_views for a ragged batch: counts[t] is the width of view t's tensors (kpts[t] [B,counts[t],2] and so on),
+ * slot_counts [batch * n_views] (device int32) the true keypoints of view t of tuple b at index b * n_views + t, clamped
+ * to [0, counts[t]].  Rows from the true count to n_pad are written as zeros, so the caller's padding (NaN included)
+ * never reaches the matcher.  slot_counts == NULL is mvm_pack_views. */
+int mvm_pack_views_ragged(const float* const* kpts, const float* const* scores, const float* const* desc,
+                          const int* counts, const int* slot_counts, int batch, int n_views, int n_pad, float* out_kpts,
+                          float* out_scores, float* out_desc, void* stream);
 
-/* Bytes of scratch mvm_matcher_forward needs for this shape. */
+/* Bytes of scratch mvm_matcher_forward needs for this shape (the capacities bound it: the same for ragged calls). */
 size_t mvm_matcher_workspace_bytes(int batch, int n_views, int n_pad, int n_pairs, int has_conf);
 
 /* MultiViewMatcher.forward in eval mode (multi_view_matcher.py:322-332; multi_match
@@ -147,6 +154,32 @@ int mvm_matcher_forward_views(const mvm_matcher_weights* w, int batch, int n_vie
                               float match_threshold, const mvm_pair_io* pairs, int n_pairs,
                               void* workspace, size_t workspace_bytes, const mvm_matcher_options* opt /* NULL = defaults */,
                               void* stream);
+
+/* mvm_matcher_forward_views for a batch whose tuples have different keypoint counts per view.  The host knows
+ * capacities, the device knows counts:
+ *   counts       HOST int[n_views]: the CAPACITY of view t (as in mvm_matcher_forward_views): it sizes every buffer and
+ *                output and picks each kernel (Sinkhorn cluster size included)
+ *   slot_counts  DEVICE int32 [batch * n_views]: the true keypoints of view t of tuple b at index b * n_views + t; the
+ *                effective count is min(max(slot_counts[i], 0), counts[t]), so no value moves an access out of bounds
+ * Inputs: rows at and past a slot's count of kpts / kscores / desc must be finite (mvm_pack_views_ragged writes zeros).
+ * Outputs keep the capacity shapes: scores [B, m_cap+1, n_cap+1], matches_a / mscores_a [B, m_cap], conf [B, m_cap, 1]
+ * and so on.  Tuple b's coupling matrix is the top-left block scores[b, :m_b+1, :n_b+1] with its dustbin row at m_b and
+ * its dustbin column at n_b: the tensor a batch-of-one call with counts m_b, n_b returns.  Past the counts matches are
+ * -1, match scores 0 and confidences 0; score entries outside the block are not written.  A -1 match gathers the
+ * tuple's last keypoint n_b - 1 and its dustbin column n_b in the confidence head, as the batch-of-one call does.
+ * A zero count is allowed: that tuple's pairs with the empty view have no matches (-1 / 0 throughout), their scores and
+ * confidences carry no meaning, and no other tuple's outputs change.
+ * Options: math_mode 3 with score_kernel 1 only (the default); math modes 0 / 1 and the fp32 CUDA-core score kernel
+ * return 1 (invalid argument) before any launch when slot_counts != NULL.  Every sinkhorn_variant is accepted (the
+ * reference / log-domain Sinkhorn entries are not on this path).  slot_counts == NULL is mvm_matcher_forward_views, bit
+ * for bit.  The workspace is mvm_matcher_workspace_bytes of the capacities, and the call is CUDA-graph capturable: one
+ * captured graph serves any device counts at the same capacities. */
+int mvm_matcher_forward_ragged(const mvm_matcher_weights* w, int batch, int n_views, int n_pad,
+                               const int* counts, const int* slot_counts, const float* kpts, const float* kscores,
+                               const float* desc, const float* view_wh, int sinkhorn_iters,
+                               float match_threshold, const mvm_pair_io* pairs, int n_pairs,
+                               void* workspace, size_t workspace_bytes, const mvm_matcher_options* opt /* NULL = defaults */,
+                               void* stream);
 
 /* ---- individual stages (exported for stage-parity tests and for callers that only need
  * one stage; same semantics as the fused forward) -------------------------------------- */
@@ -356,6 +389,12 @@ int mvm_ba2view(const float* kpts0_norm, const float* kpts1_norm, const float* c
 int mvm_gather_matches(const float* kpts, int n_views, int n_pad, const int* counts,
                        const mvm_pair_io* pairs, int n_pairs, int batch, float conf_thresh,
                        float* mkpts_a, float* mkpts_b, float* mconf, int* n_valid, void* stream);
+/* The same for the outputs of mvm_matcher_forward_ragged: counts[t] are the capacities (the row strides of matches_a /
+ * conf), slot_counts [batch * n_views] (device) bound the rows of each (tuple, pair) as in that call.  NULL =
+ * mvm_gather_matches. */
+int mvm_gather_matches_ragged(const float* kpts, int n_views, int n_pad, const int* counts, const int* slot_counts,
+                              const mvm_pair_io* pairs, int n_pairs, int batch, float conf_thresh,
+                              float* mkpts_a, float* mkpts_b, float* mconf, int* n_valid, void* stream);
 
 /* Maximum-spanning-tree initial extrinsics (bundle_adjust_io.py:135-172).  T_rel [B,P,16] relative
  * poses a->b, weight [B,P] edge weights (number of matches), success [B,P]; extr [B,T,16] doubles,
