@@ -367,7 +367,7 @@ extern "C" int mvm_ba_initialize(const int* pair_a, const int* pair_b, int n_vie
   MvmProfScope prof__(MVM_TAG_MISC, (cudaStream_t)stream);
   BaInitArgs g;
   g.n_views = n_views; g.n_pairs = n_pairs; g.batch = batch; g.n_pad = n_pad; g.min_inliers = min_inliers;
-  for (int p = 0; p < n_pairs; ++p) { g.a[p] = pair_a[p]; g.b[p] = pair_b[p]; MVM_REQUIRE(pair_a[p] < pair_b[p]); }
+  for (int p = 0; p < n_pairs; ++p) { g.a[p] = pair_a[p]; g.b[p] = pair_b[p]; MVM_REQUIRE(0 <= pair_a[p] && pair_a[p] < pair_b[p] && pair_b[p] < n_views); }
   g.extr0 = extr_tree; g.T_rel = T_rel; g.success = success; g.on_tree = on_tree; g.inliers = inliers;
   g.extr = extr_out; g.n_edges = n_edges_out;
   ba_init_kernel<<<batch, 32, 0, (cudaStream_t)stream>>>(g);

@@ -853,9 +853,9 @@ int mvm_gather_matches_ragged(const float* kpts, int n_views, int n_pad, const i
   PairTable tab;
   tab.n_pairs = n_pairs; tab.n_views = n_views; tab.slot = slot_counts;
   for (int p = 0; p < n_pairs; ++p) {
-    // the slot of a view indexes slot_counts
-    MVM_REQUIRE(!slot_counts || (pairs[p].view_a >= 0 && pairs[p].view_a < n_views && pairs[p].view_b >= 0 &&
-                                 pairs[p].view_b < n_views));
+    // a view id indexes counts (host), the views of kpts and, with slot_counts, the slots
+    MVM_REQUIRE(pairs[p].view_a >= 0 && pairs[p].view_a < n_views && pairs[p].view_b >= 0 &&
+                pairs[p].view_b < n_views);
     tab.a[p] = pairs[p].view_a; tab.b[p] = pairs[p].view_b;
     tab.m[p] = counts[pairs[p].view_a]; tab.n[p] = counts[pairs[p].view_b];
     tab.matches_a[p] = pairs[p].matches_a; tab.conf[p] = pairs[p].conf;
@@ -875,7 +875,7 @@ int mvm_spanning_tree_init(const int* pair_a, const int* pair_b, int n_views, in
   MvmProfScope prof__(MVM_TAG_MISC, (cudaStream_t)stream);
   TreeArgs t;
   t.n_views = n_views; t.n_pairs = n_pairs; t.batch = batch;
-  for (int p = 0; p < n_pairs; ++p) { t.a[p] = pair_a[p]; t.b[p] = pair_b[p]; MVM_REQUIRE(pair_a[p] < pair_b[p]); }
+  for (int p = 0; p < n_pairs; ++p) { t.a[p] = pair_a[p]; t.b[p] = pair_b[p]; MVM_REQUIRE(0 <= pair_a[p] && pair_a[p] < pair_b[p] && pair_b[p] < n_views); }
   t.T_rel = T_rel; t.weight = weight; t.success = success; t.extr = extr; t.on_tree = on_tree;
   spanning_tree_kernel<<<mvm_div_up(batch, 64), 64, 0, (cudaStream_t)stream>>>(t);
   MVM_CHECK_LAUNCH();
@@ -916,7 +916,7 @@ int mvm_multi_view_ba_obs(const int* pair_a, const int* pair_b, int n_views, int
   const int n_sm = mvm_dev_info().n_sm;
   MvbaArgs g;
   g.n_views = n_views; g.n_pairs = n_pairs; g.batch = batch; g.n_pad = n_pad;
-  for (int p = 0; p < n_pairs; ++p) { g.a[p] = pair_a[p]; g.b[p] = pair_b[p]; MVM_REQUIRE(pair_a[p] < pair_b[p]); }
+  for (int p = 0; p < n_pairs; ++p) { g.a[p] = pair_a[p]; g.b[p] = pair_b[p]; MVM_REQUIRE(0 <= pair_a[p] && pair_a[p] < pair_b[p] && pair_b[p] < n_views); }
   int groups = n_sm / n_pairs;          // one CTA per SM keeps every group co-resident
   if (groups < 1) return MVM_ERR_INVALID;
   if (groups > batch) groups = batch;
@@ -968,7 +968,7 @@ int mvm_triangulate_pairs(const int* pair_a, const int* pair_b, int n_views, int
   MvbaArgs g;
   memset(&g, 0, sizeof(g));
   g.n_views = n_views; g.n_pairs = n_pairs; g.batch = batch; g.n_pad = n_pad;
-  for (int p = 0; p < n_pairs; ++p) { g.a[p] = pair_a[p]; g.b[p] = pair_b[p]; MVM_REQUIRE(pair_a[p] < pair_b[p]); }
+  for (int p = 0; p < n_pairs; ++p) { g.a[p] = pair_a[p]; g.b[p] = pair_b[p]; MVM_REQUIRE(0 <= pair_a[p] && pair_a[p] < pair_b[p] && pair_b[p] < n_views); }
   g.xa = xn_a; g.xb = xn_b; g.n_valid = n_valid; g.extr_init = extr;
   triangulate_pairs_kernel<<<batch * n_pairs, NT, 0, stream>>>(g, points_out);
   MVM_CHECK_LAUNCH();

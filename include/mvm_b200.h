@@ -382,6 +382,12 @@ int mvm_ba2view(const float* kpts0_norm, const float* kpts1_norm, const float* c
 
 /* ---- multi-view stage (pose_optimization/multi_view/) -------------------------------- */
 
+/* Pair tables: the entries below that take pair_a / pair_b (host arrays of n_pairs view ids) require
+ * 0 <= pair_a[p] < pair_b[p] < n_views for every p and return 1 (invalid argument) before any launch
+ * otherwise: mvm_spanning_tree_init, mvm_ba_initialize, mvm_multi_view_ba(_ex/_obs) and
+ * mvm_triangulate_pairs.  mvm_gather_matches(_ragged) require 0 <= pairs[p].view_a, pairs[p].view_b < n_views
+ * in the same way. */
+
 /* Order-preserving compaction of the valid matches of every (tuple, pair):
  * valid = matches >= 0 and conf > conf_thresh (bundle_adjust_io.py:66-98, eval_pairs.py:215-222).
  * kpts [B*T, n_pad, 2]; pairs[p].matches_a / .conf are the matcher outputs of that pair.

@@ -189,6 +189,73 @@ def ba_initialize(n_views, extr_init, rel_pose):
     return np.array(out)
 
 
+def ba_initialize_edges(n_views, pairs, extr_tree, T_rel, success, on_tree, inliers, min_inliers=20):
+    """``mvm_ba_initialize`` for one tuple, edge selection included.  The pairs written to ba_init_in.csv
+    (bundle_adjust_io.py, initialize_bundle_adjust) are the edges: pair p = (a, b) is one when
+    success[p] and (its inlier count >= min_inliers or on_tree[p]).  inliers [P, n_pad] is the 0/1 inlier
+    mask of every pair, counted over all n_pad entries (None: no pair has inliers, only the tree counts).
+    If those edges do not connect every view to view 0, extr_tree is returned unchanged; otherwise
+    ba_initialize runs on them, with T_rel [P,4,4] taken as given (float32 inputs are widened to float64).
+    Returns (extrinsics [n_views,4,4], number of edges)."""
+    keep, connected = ba_init_edge_set(n_views, pairs, T_rel, success, on_tree, inliers, min_inliers)
+    if not connected:
+        return np.array(extr_tree, np.float64).copy(), len(keep)
+    return ba_initialize(n_views, np.asarray(extr_tree, np.float64), keep), len(keep)
+
+
+def ba_init_edge_set(n_views, pairs, T_rel, success, on_tree, inliers, min_inliers=20):
+    """The edge rule of ba_initialize_edges alone: ({(a, b): T_rel float64}, whether the edges reach every
+    view from view 0)."""
+    keep = {}
+    for p, (a, b) in enumerate(pairs):
+        cnt = 0 if inliers is None else int(np.asarray(inliers[p], np.int64).sum())
+        if success[p] and (cnt >= min_inliers or on_tree[p]):
+            keep[(int(a), int(b))] = np.asarray(T_rel[p], np.float64)
+    seen = {0}
+    for _ in range(n_views):
+        for a, b in keep:
+            if a in seen or b in seen:
+                seen |= {a, b}
+    return keep, len(seen) == n_views
+
+
+def make_pose_graph(seed, n_views, rot_deg=(3, 12), baseline=(0.2, 0.6), collinear=0.0, corrupt=None):
+    """Ground-truth world->cam extrinsics [n_views,4,4] (view 0 = identity) and the exact relative poses
+    T_a->b = E_b E_a^-1 of every pair a < b, as a dict.
+      rot_deg      every view v > 0 is rotated by U(rot_deg) degrees about a random axis; (130, 179) gives
+                   relative rotations past 120 deg (trace of R < 0);
+      collinear    > 0: camera centres on the x axis at 0, 1, 2, ... m, each moved off the line by at most
+                   `collinear` m (near-collinear centres); 0: centres at U(baseline) m in random directions;
+      corrupt      a pair (a, b) whose relative pose is replaced by one rotated a further 40 deg and with a
+                   translation direction turned by 90 deg (an outlier edge)."""
+    from .pose import rodrigues
+    rng = np.random.default_rng(seed)
+    extr = [np.eye(4)]
+    for v in range(1, n_views):
+        ax = rng.standard_normal(3)
+        R = rodrigues(ax / np.linalg.norm(ax) * np.deg2rad(rng.uniform(*rot_deg)))
+        if collinear > 0:
+            c = np.array([float(v), 0.0, 0.0]) + collinear * rng.uniform(-1, 1, 3)
+        else:
+            d = rng.standard_normal(3)
+            c = d / np.linalg.norm(d) * rng.uniform(*baseline)
+        E = np.eye(4)
+        E[:3, :3] = R
+        E[:3, 3] = -R @ c
+        extr.append(E)
+    extr = np.array(extr)
+    rel = {(a, b): extr[b] @ np.linalg.inv(extr[a]) for b in range(n_views) for a in range(b)}
+    if corrupt is not None:
+        ax = rng.standard_normal(3)
+        T = rel[corrupt].copy()
+        T[:3, :3] = rodrigues(ax / np.linalg.norm(ax) * np.deg2rad(40.0)) @ T[:3, :3]
+        t = T[:3, 3]
+        perp = np.cross(t, rng.standard_normal(3))
+        T[:3, 3] = perp / np.linalg.norm(perp) * np.linalg.norm(t)
+        rel[corrupt] = T
+    return extr, rel
+
+
 # ---------------------------------------------------------------------------------------------
 # the reference's known-answer scene (test_ba_init.cpp:84-91) and noise helpers (:10-49)
 # ---------------------------------------------------------------------------------------------

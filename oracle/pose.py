@@ -293,7 +293,7 @@ def _ba_residual_jacobian(T1, pts3d, x0, x1, w):
 
 
 def run_bundle_adjust_2_view(kpts0_norm, kpts1_norm, confidence, init_T021, n_iterations=10,
-                             lm_increase=1.5, lm_decrease=3.5, return_trace=False):
+                             lm_increase=1.5, lm_decrease=3.5, return_trace=False, jacobi_precond=True):
     """run_bundle_adjust_2_view (estimate_relative_pose.py:138-143) ->
     BundleAdjustGaussNewton2View.run (bundle_adjust_gauss_newton_2_view.py:127-201) with the
     defaults jacobi_precond=True, vary_lm_fact=True, non-strict checks.  Dense (6+3n)^2 solve
@@ -339,7 +339,7 @@ def run_bundle_adjust_2_view(kpts0_norm, kpts1_norm, confidence, init_T021, n_it
             if i == n_iterations:
                 break
             dA = np.diagonal(A)
-            if (dA > 0).all():                        # :171-177 Jacobi scaling
+            if jacobi_precond and (dA > 0).all():     # :171-177 Jacobi scaling
                 inv = 1.0 / np.maximum(dA, dt.type(1e-12))
                 A = inv[:, None] * A
                 bvec = inv * bvec
@@ -357,6 +357,167 @@ def run_bundle_adjust_2_view(kpts0_norm, kpts1_norm, confidence, init_T021, n_it
     if return_trace:
         return ext, valid_batch, trace
     return ext, valid_batch
+
+
+def _inv3_sym(M):
+    """Inverse of symmetric 3x3 blocks [n,3,3] by cofactors; ok [n] is False where the determinant is
+    not a non-zero number (the block is singular to float64)."""
+    a00, a01, a02 = M[:, 0, 0], M[:, 0, 1], M[:, 0, 2]
+    a11, a12, a22 = M[:, 1, 1], M[:, 1, 2], M[:, 2, 2]
+    c00 = a11 * a22 - a12 * a12
+    c01 = a02 * a12 - a01 * a22
+    c02 = a01 * a12 - a02 * a11
+    det = a00 * c00 + a01 * c01 + a02 * c02
+    ok = np.abs(det) > 0.0
+    with np.errstate(divide='ignore', invalid='ignore'):
+        idet = 1.0 / det
+        c11 = a00 * a22 - a02 * a02
+        c12 = a01 * a02 - a00 * a12
+        c22 = a00 * a11 - a01 * a01
+        inv = np.stack([np.stack([c00, c01, c02], -1), np.stack([c01, c11, c12], -1),
+                        np.stack([c02, c12, c22], -1)], -2) * idet[:, None, None]
+    return inv, ok
+
+
+def _ba_point_blocks(T1, pts, x0, x1, w):
+    """Per-point blocks of the normal equations of _ba_residual_jacobian's problem, without forming J:
+    App [n,3,3] (point), Acp [n,6,3] (camera x point), bp [n,3], and the sums Acc [6,6], bc [6] and
+    the squared residual norm."""
+    R, t = T1[:3, :3], T1[:3, 3]
+
+    def proj_jac(q):
+        iz = 1.0 / q[:, 2]
+        J = np.zeros((q.shape[0], 2, 3))
+        J[:, 0, 0] = iz
+        J[:, 1, 1] = iz
+        J[:, 0, 2] = -q[:, 0] * iz * iz
+        J[:, 1, 2] = -q[:, 1] * iz * iz
+        return w[:, None, None] * J, w[:, None] * (q[:, :2] * iz[:, None])
+
+    J0, pr0 = proj_jac(pts)
+    r0 = pr0 - w[:, None] * x0
+    q = pts @ R.T + t
+    Jpi, pr1 = proj_jac(q)
+    r1 = pr1 - w[:, None] * x1
+    J1 = Jpi @ R
+    IA = np.concatenate([np.broadcast_to(np.eye(3), (q.shape[0], 3, 3)), -hat(q)], 2)
+    Jc = Jpi @ IA                                                               # [n,2,6]
+    tr = lambda X: np.swapaxes(X, -1, -2)
+    App = tr(J0) @ J0 + tr(J1) @ J1
+    Acp = tr(Jc) @ J1
+    bp = -((tr(J0) @ r0[..., None]) + (tr(J1) @ r1[..., None]))[..., 0]
+    Acc = (tr(Jc) @ Jc).sum(0)
+    bc = -(tr(Jc) @ r1[..., None])[..., 0].sum(0)
+    rho = float((r0 ** 2).sum() + (r1 ** 2).sum())
+    return App, Acp, bp, Acc, bc, rho
+
+
+def triangulate_points_first_view_identity(T1, x0, x1, dlt='svd'):
+    """triangulate_points with P0 = [I|0], P1 = T1[:3] and one rule for a degenerate match: when the match sits
+    at the principal point of camera 0 and camera 1 observes it where camera 0's optical axis and camera 0's centre
+    both project (x0 = 0 and columns z and w of the 4x4 DLT matrix are exactly zero), the null space of the DLT
+    matrix is span(e_z, e_w) and the point is not unique.  The SVD then returns e_w, camera 0's centre, whose zero
+    depth makes the BA's Jacobians infinite; here the point is e_z, (0, 0, 1), which is what the smallest
+    eigenvector of A^T A by cyclic Jacobi gives (no rotation touches the zero rows and columns, and the first
+    smallest diagonal entry wins).  x0, x1 [n,2] -> [n,3] float64.
+
+    dlt='normal' takes the smallest eigenvector of A^T A instead of the smallest right-singular vector of A: the
+    same point in exact arithmetic, but its rounding error grows with cond(A)^2 instead of cond(A), which is what a
+    solver working on A^T A (as the CUDA kernels do) carries on near-parallel rays."""
+    R, t = T1[:3, :3], T1[:3, 3]
+    if dlt == 'svd':
+        X = triangulate_points(np.eye(4)[:3][None], T1[None, :3], x0[None], x1[None])[0]
+    else:
+        assert dlt == 'normal', dlt
+        A = np.zeros((x0.shape[0], 4, 4))
+        A[:, 0, 0] = A[:, 1, 1] = -1.0
+        A[:, 0, 2], A[:, 1, 2] = x0[:, 0], x0[:, 1]
+        A[:, 2, :3] = x1[:, 0:1] * R[2] - R[0]
+        A[:, 3, :3] = x1[:, 1:2] * R[2] - R[1]
+        A[:, 2, 3], A[:, 3, 3] = x1[:, 0] * t[2] - t[0], x1[:, 1] * t[2] - t[1]
+        h = np.linalg.eigh(np.swapaxes(A, 1, 2) @ A)[1][:, :, 0]
+        X = convert_points_from_homogeneous(h)
+    colz = np.stack([x0[:, 0], x0[:, 1], x1[:, 0] * R[2, 2] - R[0, 2], x1[:, 1] * R[2, 2] - R[1, 2]], 1)
+    colw = np.stack([x1[:, 0] * t[2] - t[0], x1[:, 1] * t[2] - t[1]], 1)
+    tie = ~colz.any(1) & ~colw.any(1)
+    X[tie] = [0.0, 0.0, 1.0]
+    return X
+
+
+def run_bundle_adjust_2_view_schur(kpts0_norm, kpts1_norm, confidence, init_T021, n_iterations=10,
+                                   lm_increase=1.5, lm_decrease=3.5, jacobi_precond=True, dlt='svd'):
+    """run_bundle_adjust_2_view in float64 with the 3x3 point blocks eliminated (Schur complement)
+    instead of the dense (6+3n)^2 solve: the same LM iteration at any n.
+
+    For every item: valid matches conf > 0, excluded (T_init returned) with <= 6 of them; weights
+    conf / (0.5 * max(sum over the 2n observations, 1e-6)); points triangulated with T_init; n_iterations+1
+    evaluations of the squared residual norm (the trace), lambda0 = 0.1, lambda / lm_decrease on a new
+    best residual and * lm_increase otherwise; each step solves (A + lambda D) delta = b with D = max(diag A,
+    1e-12) when every diagonal entry is positive (Jacobi scaling) and D = I otherwise, and is applied
+    unconditionally; the best evaluated pose is returned.  The points are triangulated by
+    triangulate_points_first_view_identity (a match on both optical axes of a forward motion becomes (0, 0, 1);
+    dlt selects its solver).  A step is skipped (nothing moves) when a damped
+    point block has a zero determinant, when the 6x6 camera system is singular, or when its solution is
+    not finite.
+
+    Returns (T_out [B,4,4] with T_init for excluded items, valid [B], trace: a list with an
+    [n_iterations+1] array per item, None for excluded ones)."""
+    B = kpts0_norm.shape[0]
+    conf = confidence[..., 0] if confidence.ndim == 3 else confidence
+    T_out = np.array(init_T021, np.float64).copy()
+    valid_batch = np.zeros(B, bool)
+    traces = []
+    for b in range(B):
+        mk = conf[b] > 0
+        if mk.sum() <= 6:
+            traces.append(None)
+            continue
+        valid_batch[b] = True
+        x0 = np.asarray(kpts0_norm[b][mk], np.float64)
+        x1 = np.asarray(kpts1_norm[b][mk], np.float64)
+        c = np.asarray(conf[b][mk], np.float64)
+        w = c / (0.5 * max(2.0 * c.sum(), 1e-6))
+        T1 = np.array(init_T021[b], np.float64).copy()
+        T1[3] = [0, 0, 0, 1]
+        pts = triangulate_points_first_view_identity(T1, x0, x1, dlt)
+        best_T, best_r, lam = T1.copy(), None, 0.1
+        tr = []
+        for i in range(n_iterations + 1):
+            App, Acp, bp, Acc, bc, rn = _ba_point_blocks(T1, pts, x0, x1, w)
+            tr.append(rn)
+            if i == 0:
+                best_r, best_T = rn, T1.copy()
+            elif rn < best_r:
+                best_r, best_T = rn, T1.copy()
+                lam = lam / lm_decrease
+            else:
+                lam = lam * lm_increase
+            if i == n_iterations:
+                break
+            dP = np.diagonal(App, axis1=1, axis2=2)
+            dC = np.diagonal(Acc)
+            if jacobi_precond and (dP > 0).all() and (dC > 0).all():
+                Dp, Dc = np.maximum(dP, 1e-12), np.maximum(dC, 1e-12)
+            else:
+                Dp, Dc = np.ones_like(dP), np.ones(6)
+            Mi, ok = _inv3_sym(App + lam * Dp[:, :, None] * np.eye(3))
+            if not ok.all():
+                continue
+            Y = Acp @ Mi                                                    # [n,6,3]
+            S = Acc - (Y @ np.swapaxes(Acp, 1, 2)).sum(0) + lam * np.diag(Dc)
+            g = bc - (Y @ bp[..., None])[..., 0].sum(0)
+            try:
+                dc = np.linalg.solve(S, g)
+            except np.linalg.LinAlgError:
+                continue
+            if not np.isfinite(dc).all():
+                continue
+            dp = (Mi @ (bp - (np.swapaxes(Acp, 1, 2) @ dc))[..., None])[..., 0]
+            T1 = se3_exp_map_T(dc[None])[0] @ T1
+            pts = pts + dp
+        T_out[b] = best_T
+        traces.append(np.array(tr))
+    return T_out, valid_batch, traces
 
 
 # ----------------------------------------------------------------------------------------
@@ -407,18 +568,33 @@ def rodrigues(w):
 
 
 def make_two_view_scene(seed, n, outlier_frac=0.3, noise_px=1.0, width=640, height=480,
-                        f=577.87, dtype=np.float32):
-    """3-D points in the frustum of camera 0 (depth 1..5 m), camera 1 rotated <= 30 deg about a
-    random axis with a 0.1..1 m baseline, K = [[f,0,319.5],[0,f,239.5],[0,0,1]], 1 px noise,
-    30 % outlier matches, confidences U(0.5,1) inliers / U(0,0.3) outliers."""
+                        f=577.87, dtype=np.float32, motion='random', rot_deg=(5, 30)):
+    """3-D points in the frustum of camera 0 (depth 1..5 m), K = [[f,0,319.5],[0,f,239.5],[0,0,1]],
+    1 px noise, 30 % outlier matches, confidences U(0.5,1) inliers / U(0,0.3) outliers.  Camera 1:
+      motion='random'  rotated by U(rot_deg) degrees (default 5..30) about a random axis, 0.1..1 m
+                       baseline in a random direction (the defaults give the scenes this function
+                       has always produced);
+      motion='forward' rotated by U(rot_deg) degrees, centre 0.1..0.5 m straight ahead of camera 0
+                       (rot_deg=(0, 0): pure forward motion, the epipole at the principal point);
+      motion='orbit'   rotated by U(rot_deg) degrees about an axis in camera 0's image plane and
+                       looking at the point 3 m ahead of camera 0 from 3 m away: relative rotations
+                       past 90 deg (e.g. rot_deg=(130, 179)) with every point in front of both."""
     rng = np.random.default_rng(seed)
     K = np.array([[f, 0, (width - 1) / 2], [0, f, (height - 1) / 2], [0, 0, 1]], np.float64)
     axis = rng.standard_normal(3)
+    if motion == 'orbit':
+        axis[2] = 0.0
     axis /= np.linalg.norm(axis)
-    R = rodrigues(axis * np.deg2rad(rng.uniform(5, 30)))
+    R = rodrigues(axis * np.deg2rad(rng.uniform(*rot_deg)))
     tdir = rng.standard_normal(3)
     tdir /= np.linalg.norm(tdir)
     t = tdir * rng.uniform(0.1, 1.0)
+    if motion == 'forward':
+        t = -R @ np.array([0.0, 0.0, rng.uniform(0.1, 0.5)])
+    elif motion == 'orbit':
+        t = np.array([0.0, 0.0, 3.0]) - R @ np.array([0.0, 0.0, 3.0])
+    else:
+        assert motion == 'random', motion
     T = np.eye(4)
     T[:3, :3], T[:3, 3] = R, t
     pts0, pts1 = [], []
