@@ -70,6 +70,21 @@ def _log_optimal_transport(scores, alpha, iters):
     return Z + u.unsqueeze(2) + v.unsqueeze(1) - norm
 
 
+def confidence_head(sd, mdesc0, mdesc1, scores, indices0):
+    """ConfidenceMLP and its call site (multi_view_matcher.py:39-53, :302-306) in the dtype of mdesc0: the conf_mlp
+    weights of `sd` (torch tensors) are cast to it.  mdesc0 [B, 256, m], mdesc1 [B, 256, n], scores [B, m+1, n+1],
+    indices0 [B, m] (int64, -1 = no match: gathers the last keypoint of view 1 and the dustbin column).
+    Returns [B, m, 1]."""
+    dt, dev = mdesc0.dtype, mdesc0.device
+    sd = {k: (v.to(dev, dt) if v.is_floating_point() else v) for k, v in sd.items() if k.startswith('conf_mlp.')}
+    bi = torch.arange(indices0.shape[0], device=dev).unsqueeze(-1).repeat(1, indices0.shape[-1])
+    add = scores.to(dt)[bi, torch.arange(indices0.shape[-1], device=dev), indices0].unsqueeze(-2)
+    g1 = mdesc1.transpose(-2, -1)[bi, indices0].transpose(-2, -1)
+    of = _mlp(sd, 'conf_mlp.layers_f', [512, 512, 256], torch.cat([mdesc0, g1], -2), last_layer=False)
+    oc = _mlp(sd, 'conf_mlp.layers_c', [1, 256, 256], add, last_layer=False)
+    return torch.sigmoid(_mlp(sd, 'conf_mlp.layers', [256, 1], of + oc)).transpose(-2, -1)
+
+
 def matcher_forward(sd_np, config, data_np, device=None, to_numpy=True):
     """MultiViewMatcher.forward (eval, multi_frame_matching=True branch or pairwise) -> numpy dict."""
     dev = torch.device(device) if device is not None else torch.device('cpu')
@@ -106,12 +121,7 @@ def matcher_forward(sd_np, config, data_np, device=None, to_numpy=True):
             v1 = mut1 & v0.gather(1, i1)
             i0 = torch.where(v0, i0, i0.new_tensor(-1))
             i1 = torch.where(v1, i1, i1.new_tensor(-1))
-            bi = torch.arange(i0.shape[0], device=dev).unsqueeze(-1).repeat(1, i0.shape[-1])
-            add = sc[bi, torch.arange(i0.shape[-1], device=dev), i0].unsqueeze(-2)
-            g1 = m1.transpose(-2, -1)[bi, i0].transpose(-2, -1)
-            of = _mlp(sd, 'conf_mlp.layers_f', [512, 512, 256], torch.cat([m0, g1], -2), last_layer=False)
-            oc = _mlp(sd, 'conf_mlp.layers_c', [1, 256, 256], add, last_layer=False)
-            conf = torch.sigmoid(_mlp(sd, 'conf_mlp.layers', [256, 1], of + oc)).transpose(-2, -1)
+            conf = confidence_head(sd, m0, m1, sc, i0)
             res['matches%d_%d_%d' % (a, a, b)] = out(i0)
             res['matches%d_%d_%d' % (b, a, b)] = out(i1)
             res['matching_scores%d_%d_%d' % (a, a, b)] = out(ms0)
